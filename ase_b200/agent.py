@@ -687,7 +687,7 @@ class CommonAgent:
                     raise RuntimeError(f"epoch {r['epoch']}: a peer rank did not reach the gradient barrier of the multi-GPU optimizer step within ~15 s "
                                        "(csrc/peer.cu); that update was skipped -- restore() the last checkpoint")
                 if status != 0:
-                    raise RuntimeError(f"epoch {r['epoch']}: FP16 operand-plane scale miss -- a tensor's max moved by more than 2^9 up / 2^12 down between "
+                    raise RuntimeError(f"epoch {r['epoch']}: FP16 operand-plane scale miss -- a tensor's max moved by more than ~2^7 up / ~2^14 down between "
                                        "two consecutive calls; rerun with gemm_backend=1 (restore() the last checkpoint)")
                 rs, ls, cnt = (r['scalars'].pop(k, 0.0) for k in ('ep_reward_sum', 'ep_length_sum', 'ep_count'))
                 if cnt > 0:       # common_agent.py:125-136 (mean over the episodes that finished in this epoch)

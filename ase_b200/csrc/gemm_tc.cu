@@ -597,7 +597,7 @@ tc_site_update_kernel(unsigned* __restrict__ amax, float* __restrict__ scale, in
   const float a = __uint_as_float(amax[i]);
   const float s0 = scale[2 * i];
   if (a > 0.0f) {
-    if (s0 != 0.0f && a * s0 < 0.015625f) atomicOr(flag, 2u);        // the tensor shrank by > 2^12 between two calls: the split lost bits
+    if (s0 != 0.0f && a * s0 < 0.015625f) atomicOr(flag, 2u);        // the tensor shrank by > 2^14 .. 2^15 since the last call: the split lost bits
     const float s = scale_from_amax(a, TOP_SITE);
     scale[2 * i] = s; scale[2 * i + 1] = 1.0f / s;
     amax[i] = 0u;

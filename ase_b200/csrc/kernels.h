@@ -38,8 +38,11 @@ struct PlaneBuf {
 // one slot per SITE = (GEMM index within the top-level call, operand A / B / output C): the static kernel schedule of the learner
 // puts the same logical tensor at the same site every call.  The first time a site is used its scale comes from an exact max pass
 // (or from the max the producing GEMM tracked); afterwards the scale predicted from the previous call's max is used, which lets the
-// producing GEMM's epilogue write the planes itself.  The prediction leaves 2^9 of headroom above and 2^12 below; leaving that
-// window between two consecutive calls raises a sticky device flag (ase_learner_plane_status), never a silent wrong result.
+// producing GEMM's epilogue write the planes itself.  The predicted scale puts the previous call's max into [2^8, 2^9).  Overflow: a
+// scaled value above 60000, i.e. growth by more than x117 .. x234 (never flagged at x64, always at x512), is flagged by the writer in
+// the same call.  Underflow: a scaled max below 2^-6, i.e. shrinking by more than 2^14 .. 2^15 (never flagged at 2^-13, always at
+// 2^-16), is flagged by tc_site_update_kernel at the start of the NEXT call.  Either raises a sticky device flag
+// (ase_learner_plane_status), never a silent wrong result (tests/test_gpu_learner_shapes.py pins both edges).
 struct TcPrepItem { const float* src; void* hi; void* lo; int rows, cols, ldp, site, buf; };
 struct TcPrepBatch { static constexpr int MAX = 40; TcPrepItem item[MAX]; };
 struct PlaneRegistry {

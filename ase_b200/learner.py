@@ -279,7 +279,7 @@ class Learner:
             raise L.AseError("multi-GPU optimizer step: a peer rank did not reach the gradient barrier within ~15 s (csrc/peer.cu); the update was skipped")
         if f.value:
             raise L.AseError(f"FP16 operand-plane scale miss (flags {f.value}: bit0 overflow, bit1 underflow): a tensor's max moved by more "
-                             "than 2^9 up / 2^12 down between two consecutive calls; rerun with gemm_backend=1")
+                             "than ~2^7 up / ~2^14 down between two consecutive calls; rerun with gemm_backend=1")
         return 0
 
     def plane_flag_to(self, dst):

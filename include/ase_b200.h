@@ -316,9 +316,13 @@ typedef struct {
  * initialisation, broadcast): the tensor-core backends cache hi/lo planes of the weights between calls. */
 int ase_learner_params_changed(AseLearner* l);
 /* gemm_backend 2 (scaled FP16 operand planes): sticky status of the per-tensor power-of-two scales, read with one
- * stream synchronisation.  0 = fine.  Bit 0: a value did not fit the scale predicted from the previous call (> 2^9 growth of a
- * tensor's max between two consecutive calls); bit 1: a tensor's max shrank by > 2^12 between two calls (its split lost
- * precision).  Either means the results of the flagged call are not fp32-accurate: the host mirror raises. */
+ * stream synchronisation.  0 = fine.  Bit 0: a value did not fit the scale predicted from the previous call (a tensor's max grew
+ * by more than x117 .. x234 between two consecutive calls; x64 always fits); reported after the call that overflowed.  Bit 1: a
+ * tensor's max shrank by more than 2^14 .. 2^15 between two calls (2^-13 always fits), so its split lost precision; this is
+ * detected when the next call starts, so it is reported after the call FOLLOWING the one that shrank.  That lag is accepted: the
+ * flag is sticky and the agent reads it once per epoch, and an underflowed split loses precision gradually (at the flagging edge
+ * the max still keeps about 16 bits) instead of saturating as an overflow does.  Either bit means results since the last clear are
+ * not fp32-accurate: the host mirror raises. */
 int ase_learner_plane_status(AseLearner* l, int* flags, void* stream);
 /* The same flag without a host round trip: dst[i * stride] = (float)flags for i < count, on the stream (the agent lets it ride in its
  * per-epoch train_result record); ..._clear resets it after the host has dealt with a miss. */

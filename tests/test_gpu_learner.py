@@ -152,8 +152,10 @@ def test_calc_gradients_vs_reference_golden_simt(name):
 
 
 @pytest.mark.parametrize('backend', [1, 2])      # 1: 3xTF32 planes, 2: 3xFP16 scaled planes
-@pytest.mark.parametrize('name', ['calc_grad_ase_cfg1.pt', 'calc_grad_amp_cfg.pt'])
-def test_calc_gradients_vs_reference_golden_tcgen05(name, backend):
+@pytest.mark.parametrize('name', ['calc_grad_ase_small.pt', 'calc_grad_ase_cfg1.pt', 'calc_grad_amp_cfg.pt'])
+def test_calc_gradients_vs_reference_golden_tensor_core(name, backend):
+    """calc_grad_ase_small.pt has ragged widths (trunks 64 / 48 / 32, disc 48 / 40 / 24) and B = 64, Ba = 16: tiles narrower than 128
+    and M tails in every GEMM of the wgmma learner."""
     import ctypes as C
     from ase_b200 import lib as L
     L.lib.ase_gemm_tc_profile(1)
@@ -257,7 +259,7 @@ def test_inference_with_shipped_checkpoint_statistics_vs_reference_golden(backen
 
 def test_fp16_plane_scale_miss_is_reported():
     """gemm_backend 2 predicts each tensor's power-of-two scale from the previous call.  A tensor whose max jumps by more than
-    2^9 between two calls cannot be represented: the library must say so (sticky flag -> AseError), never return silently wrong
+    x117 .. x234 between two calls cannot be represented (tests/test_gpu_learner_shapes.py pins the edges): the library must say so (sticky flag -> AseError), never return silently wrong
     gradients; after the parameters are re-announced the scales are re-derived exactly and the same input is fine."""
     from ase_b200 import Learner, lib as L
     B = 192
