@@ -207,6 +207,109 @@ heading_reward_kernel(const float* __restrict__ pos, int64_t ps, const float* __
   reward[e] = 0.7f * dir_reward + 0.3f * facing;
 }
 
+// F.normalize(tar_xy - root_xy) (eps 1e-12: a target exactly at the root gives a zero direction) and the velocity-toward-target term
+// shared by compute_location_reward (humanoid_location.py:196-210) and compute_strike_reward (humanoid_strike.py:232-244)
+__device__ __forceinline__ float toward_target_vel_reward(const float* p, const float* pp, float dx, float dy, float tar_speed, float dt,
+                                                          float* tdx, float* tdy) {
+  const float inv = 1.0f / fmaxf(sqrtf(dx * dx + dy * dy), 1e-12f);
+  const float tx = dx * inv, ty = dy * inv;
+  const float vx = (p[0] - pp[0]) / dt, vy = (p[1] - pp[1]) / dt;
+  const float tar_dir_speed = tx * vx + ty * vy;
+  const float err = fmaxf(tar_speed - tar_dir_speed, 0.0f);
+  *tdx = tx; *tdy = ty;
+  return tar_dir_speed <= 0.0f ? 0.0f : expf(-4.0f * (err * err));
+}
+
+// env/tasks/humanoid_location.py:169-182: 2-d target (z = 0) relative to the root, rotated by the inverse heading, xy kept
+__global__ void __launch_bounds__(128)
+location_obs_kernel(const float* __restrict__ root, int64_t rs, const float* __restrict__ tar, int n, float* __restrict__ obs, int64_t ld, int col0) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n) return;
+  const float* r = root + (int64_t)e * rs;
+  const Quat hq = calc_heading_quat_inv({r[3], r[4], r[5], r[6]});
+  const Vec3 d = {tar[2 * e] - r[0], tar[2 * e + 1] - r[1], 0.0f - r[2]};
+  const Vec3 l = quat_rotate(hq, d);
+  float* o = obs + (int64_t)e * ld + col0;
+  o[0] = l.x; o[1] = l.y;
+}
+
+// env/tasks/humanoid_location.py:184-228
+__global__ void __launch_bounds__(128)
+location_reward_kernel(const float* __restrict__ root, int64_t rs, const float* __restrict__ prev, int64_t pps, const float* __restrict__ tar,
+                       float tar_speed, float dt, int n, float* __restrict__ reward) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n) return;
+  const float* r = root + (int64_t)e * rs;
+  const float dx = tar[2 * e] - r[0], dy = tar[2 * e + 1] - r[1];
+  const float pos_err = dx * dx + dy * dy;
+  const float pos_reward = expf(-0.5f * pos_err);
+  float tx, ty;
+  float vel_reward = toward_target_vel_reward(r, prev + (int64_t)e * pps, dx, dy, tar_speed, dt, &tx, &ty);
+  const Quat hq = calc_heading_quat({r[3], r[4], r[5], r[6]});
+  const Vec3 f = quat_rotate(hq, {1.0f, 0.0f, 0.0f});
+  float facing_reward = fmaxf(tx * f.x + ty * f.y, 0.0f);
+  if (pos_err < 0.5f) { facing_reward = 1.0f; vel_reward = 1.0f; }     // dist_mask
+  reward[e] = 0.5f * pos_reward + 0.4f * vel_reward + 0.1f * facing_reward;
+}
+
+// env/tasks/humanoid_reach.py:174-182: the ABSOLUTE target rotated by the inverse heading (the root position is not subtracted, sic)
+__global__ void __launch_bounds__(128)
+reach_obs_kernel(const float* __restrict__ root, int64_t rs, const float* __restrict__ tar, int n, float* __restrict__ obs, int64_t ld, int col0) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n) return;
+  const float* r = root + (int64_t)e * rs;
+  const Quat hq = calc_heading_quat_inv({r[3], r[4], r[5], r[6]});
+  const Vec3 l = quat_rotate(hq, {tar[3 * e], tar[3 * e + 1], tar[3 * e + 2]});
+  float* o = obs + (int64_t)e * ld + col0;
+  o[0] = l.x; o[1] = l.y; o[2] = l.z;
+}
+
+// env/tasks/humanoid_reach.py:184-195: exp(-4 |tar - reach_body_pos|^2)
+__global__ void __launch_bounds__(128)
+reach_reward_kernel(const float* __restrict__ body, int64_t es, int64_t bs, int reach_body, const float* __restrict__ tar, int n,
+                    float* __restrict__ reward) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n) return;
+  const float* b = body + (int64_t)e * es + (int64_t)reach_body * bs;
+  const float dx = tar[3 * e] - b[0], dy = tar[3 * e + 1] - b[1], dz = tar[3 * e + 2] - b[2];
+  reward[e] = expf(-4.0f * (dx * dx + dy * dy + dz * dz));
+}
+
+// env/tasks/humanoid_strike.py:193-216: local pos (z := the target's absolute z before the rotation, sic) | tan_norm | vel | ang vel
+__global__ void __launch_bounds__(128)
+strike_obs_kernel(const float* __restrict__ root, int64_t rs, const float* __restrict__ tar, int64_t ts, int n, float* __restrict__ obs,
+                  int64_t ld, int col0) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n) return;
+  const float* r = root + (int64_t)e * rs;
+  const float* t = tar + (int64_t)e * ts;
+  const Quat hq = calc_heading_quat_inv({r[3], r[4], r[5], r[6]});
+  const Vec3 lp = quat_rotate(hq, {t[0] - r[0], t[1] - r[1], t[2]});
+  const Vec3 lv = quat_rotate(hq, {t[7], t[8], t[9]}), lw = quat_rotate(hq, {t[10], t[11], t[12]});
+  float* o = obs + (int64_t)e * ld + col0;
+  o[0] = lp.x; o[1] = lp.y; o[2] = lp.z;
+  quat_to_tan_norm(quat_mul(hq, {t[3], t[4], t[5], t[6]}), o + 3);
+  o[9] = lv.x; o[10] = lv.y; o[11] = lv.z;
+  o[12] = lw.x; o[13] = lw.y; o[14] = lw.z;
+}
+
+// env/tasks/humanoid_strike.py:218-251 (strike_body_vel and near_dist are parameters there but unused)
+__global__ void __launch_bounds__(128)
+strike_reward_kernel(const float* __restrict__ tar, int64_t ts, const float* __restrict__ root, int64_t rs, const float* __restrict__ prev,
+                     int64_t pps, float dt, int n, float* __restrict__ reward) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n) return;
+  const float* t = tar + (int64_t)e * ts;
+  const float* r = root + (int64_t)e * rs;
+  const Vec3 tar_up = quat_rotate({t[3], t[4], t[5], t[6]}, {0.0f, 0.0f, 1.0f});
+  const float tar_rot_err = tar_up.z;
+  const float tar_rot_r = fmaxf(1.0f - tar_rot_err, 0.0f);
+  float tx, ty;
+  const float vel_reward = toward_target_vel_reward(r, prev + (int64_t)e * pps, t[0] - r[0], t[1] - r[1], 1.0f, dt, &tx, &ty);
+  const float rew = 0.6f * tar_rot_r + 0.4f * vel_reward;
+  reward[e] = tar_rot_err < 0.2f ? 1.0f : rew;                         // succ
+}
+
 }  // namespace ase
 
 using namespace ase;
@@ -229,6 +332,64 @@ extern "C" int ase_heading_reward(const float* root_pos, int64_t root_pos_stride
   heading_reward_kernel<<<ceil_div(num_envs, 128), 128, 0, (cudaStream_t)stream>>>(root_pos, root_pos_stride, prev_root_pos, prev_stride,
                                                                                     root_rot, rot_stride, tar_dir, tar_speed, tar_face_dir, dt,
                                                                                     num_envs, reward);
+  ASE_LAUNCH_OK();
+  return ASE_OK;
+}
+
+extern "C" int ase_location_obs(const float* root_states, int64_t root_stride, const float* tar_pos, int num_envs, float* obs, int64_t obs_ld,
+                                int obs_col0, void* stream) {
+  ASE_CHECK_ARG(root_states && tar_pos && obs, "ase_location_obs: null pointer");
+  if (num_envs <= 0) return ASE_OK;
+  location_obs_kernel<<<ceil_div(num_envs, 128), 128, 0, (cudaStream_t)stream>>>(root_states, root_stride, tar_pos, num_envs, obs, obs_ld, obs_col0);
+  ASE_LAUNCH_OK();
+  return ASE_OK;
+}
+
+extern "C" int ase_location_reward(const float* root_states, int64_t root_stride, const float* prev_root_pos, int64_t prev_stride, const float* tar_pos,
+                                   float tar_speed, float dt, int num_envs, float* reward, void* stream) {
+  ASE_CHECK_ARG(root_states && prev_root_pos && tar_pos && reward, "ase_location_reward: null pointer");
+  if (num_envs <= 0) return ASE_OK;
+  location_reward_kernel<<<ceil_div(num_envs, 128), 128, 0, (cudaStream_t)stream>>>(root_states, root_stride, prev_root_pos, prev_stride, tar_pos,
+                                                                                     tar_speed, dt, num_envs, reward);
+  ASE_LAUNCH_OK();
+  return ASE_OK;
+}
+
+extern "C" int ase_reach_obs(const float* root_states, int64_t root_stride, const float* tar_pos, int num_envs, float* obs, int64_t obs_ld,
+                             int obs_col0, void* stream) {
+  ASE_CHECK_ARG(root_states && tar_pos && obs, "ase_reach_obs: null pointer");
+  if (num_envs <= 0) return ASE_OK;
+  reach_obs_kernel<<<ceil_div(num_envs, 128), 128, 0, (cudaStream_t)stream>>>(root_states, root_stride, tar_pos, num_envs, obs, obs_ld, obs_col0);
+  ASE_LAUNCH_OK();
+  return ASE_OK;
+}
+
+extern "C" int ase_reach_reward(const float* body_state, int64_t env_stride, int64_t body_stride, int reach_body, const float* tar_pos, int num_envs,
+                                float* reward, void* stream) {
+  ASE_CHECK_ARG(body_state && tar_pos && reward && reach_body >= 0, "ase_reach_reward: bad argument");
+  if (num_envs <= 0) return ASE_OK;
+  reach_reward_kernel<<<ceil_div(num_envs, 128), 128, 0, (cudaStream_t)stream>>>(body_state, env_stride, body_stride, reach_body, tar_pos, num_envs,
+                                                                                  reward);
+  ASE_LAUNCH_OK();
+  return ASE_OK;
+}
+
+extern "C" int ase_strike_obs(const float* root_states, int64_t root_stride, const float* tar_states, int64_t tar_stride, int num_envs, float* obs,
+                              int64_t obs_ld, int obs_col0, void* stream) {
+  ASE_CHECK_ARG(root_states && tar_states && obs, "ase_strike_obs: null pointer");
+  if (num_envs <= 0) return ASE_OK;
+  strike_obs_kernel<<<ceil_div(num_envs, 128), 128, 0, (cudaStream_t)stream>>>(root_states, root_stride, tar_states, tar_stride, num_envs, obs, obs_ld,
+                                                                                obs_col0);
+  ASE_LAUNCH_OK();
+  return ASE_OK;
+}
+
+extern "C" int ase_strike_reward(const float* tar_states, int64_t tar_stride, const float* root_states, int64_t root_stride, const float* prev_root_pos,
+                                 int64_t prev_stride, float dt, int num_envs, float* reward, void* stream) {
+  ASE_CHECK_ARG(tar_states && root_states && prev_root_pos && reward, "ase_strike_reward: null pointer");
+  if (num_envs <= 0) return ASE_OK;
+  strike_reward_kernel<<<ceil_div(num_envs, 128), 128, 0, (cudaStream_t)stream>>>(tar_states, tar_stride, root_states, root_stride, prev_root_pos,
+                                                                                   prev_stride, dt, num_envs, reward);
   ASE_LAUNCH_OK();
   return ASE_OK;
 }

@@ -349,6 +349,101 @@ humanoid_reset_kernel(const int64_t* __restrict__ progress, const float* __restr
   }
 }
 
+// env/tasks/humanoid_strike.py:254-295 compute_humanoid_reset: the base rule plus "the target was hit while a body other than the strike bodies
+// touches something".  nonstrike_body_force aliases masked_contact_buf, but fall_contact is computed before the strike bodies are zeroed.
+__global__ void __launch_bounds__(256)
+strike_reset_kernel(const int64_t* __restrict__ progress, const float* __restrict__ contact, int64_t contact_env_stride, int64_t contact_body_stride,
+                    const float* __restrict__ body_state, int64_t env_stride, int64_t body_stride, int J, const uint8_t* __restrict__ is_contact_body,
+                    const uint8_t* __restrict__ is_strike_body, const float* __restrict__ term_heights, const float* __restrict__ tar_contact,
+                    int64_t tar_contact_stride, float max_episode_length, int early_term, int n, uint8_t* __restrict__ reset_out,
+                    uint8_t* __restrict__ terminate_out) {
+  const int e = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (e >= n) return;
+  int fc = 0, fh = 0, ns = 0;
+  if (early_term) {
+    for (int b = lane; b < J; b += 32) {
+      if (is_contact_body[b]) continue;
+      const float* c = contact + (int64_t)e * contact_env_stride + (int64_t)b * contact_body_stride;
+      fc |= (fabsf(c[0]) > 0.1f) || (fabsf(c[1]) > 0.1f) || (fabsf(c[2]) > 0.1f);
+      fh |= body_state[(int64_t)e * env_stride + (int64_t)b * body_stride + 2] < term_heights[b];
+      if (!is_strike_body[b]) ns |= (fabsf(c[0]) > 1.0f) || (fabsf(c[1]) > 1.0f) || (fabsf(c[2]) > 1.0f);
+    }
+  }
+  fc = __any_sync(0xffffffffu, fc); fh = __any_sync(0xffffffffu, fh); ns = __any_sync(0xffffffffu, ns);
+  if (lane == 0) {
+    const int64_t p = progress[e];
+    int term = 0;
+    if (early_term) {
+      const float* tc = tar_contact + (int64_t)e * tar_contact_stride;
+      const bool tar_has_contact = (fabsf(tc[0]) > 1.0f) || (fabsf(tc[1]) > 1.0f);      // x and y only
+      term = ((fc && fh) || (tar_has_contact && ns)) && p > 1;
+    }
+    terminate_out[e] = (uint8_t)term;
+    reset_out[e] = (uint8_t)(((float)p >= max_episode_length - 1.0f) ? 1 : term);
+  }
+}
+
+// _update_task / _reset_task of humanoid_{heading,location,reach}.py and _reset_target of humanoid_strike.py, mask driven.  One thread per env.
+// Update mode (mask NULL): envs with progress >= change_steps resample.  Reset mode: envs with a non-zero mask resample.  Uniform k of an env is
+// its k-th draw in the reference's order (torch.rand calls, or the columns of torch.rand([n, c])); the randint of change_steps is [min, max).
+__global__ void __launch_bounds__(128)
+task_resample_kernel(AseTaskParams p, const float* __restrict__ root, int64_t rs, const int64_t* __restrict__ progress, const uint8_t* __restrict__ mask,
+                     int n, float* __restrict__ tar, int64_t ts, float* __restrict__ tar_speed, float* __restrict__ face, int64_t* __restrict__ change_steps,
+                     const uint64_t* __restrict__ rng, int sid, const float* __restrict__ u_in, const int64_t* __restrict__ steps_in) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n) return;
+  const bool go = mask ? mask[e] != 0 : progress[e] >= change_steps[e];
+  if (!go) return;
+  float u[4];
+  if (u_in) {
+    for (int q = 0; q < 4; ++q) u[q] = u_in[(int64_t)e * 4 + q];
+  } else {
+    const uint4 r = philox_u4(rng, (uint32_t)sid, (uint32_t)e, 0u);
+    u[0] = u01(r.x); u[1] = u01(r.y); u[2] = u01(r.z); u[3] = u01(r.w);
+  }
+  const float kTwoPi = 6.28318530717958647692f, kPi = 3.14159265358979323846f;
+  const float* r = root + (int64_t)e * rs;
+  float* t = tar + (int64_t)e * ts;
+  // __f*_rn: the reference rounds each product and sum separately (no fused multiply-add)
+  switch (p.kind) {
+    case ASE_TASK_HEADING: {                      // humanoid_heading.py:154-174
+      float th = 0.0f, thf = 0.0f;
+      int k = 0;
+      if (p.rand_heading) { th = __fsub_rn(__fmul_rn(kTwoPi, u[0]), kPi); thf = __fsub_rn(__fmul_rn(kTwoPi, u[1]), kPi); k = 2; }
+      tar_speed[e] = __fadd_rn(__fmul_rn(p.speed_max - p.speed_min, u[k]), p.speed_min);
+      t[0] = cosf(th); t[1] = sinf(th);
+      face[2 * e] = cosf(thf); face[2 * e + 1] = sinf(thf);
+      break;
+    }
+    case ASE_TASK_LOCATION:                       // humanoid_location.py:115-125: root xy + dist_max * (2u - 1)
+      t[0] = __fadd_rn(r[0], __fmul_rn(p.dist_max, __fsub_rn(2.0f * u[0], 1.0f)));
+      t[1] = __fadd_rn(r[1], __fmul_rn(p.dist_max, __fsub_rn(2.0f * u[1], 1.0f)));
+      break;
+    case ASE_TASK_REACH:                          // humanoid_reach.py:119-130: absolute xy, height in [min, max)
+      t[0] = __fmul_rn(p.dist_max, __fsub_rn(2.0f * u[0], 1.0f));
+      t[1] = __fmul_rn(p.dist_max, __fsub_rn(2.0f * u[1], 1.0f));
+      t[2] = __fadd_rn(__fmul_rn(p.height_max - p.height_min, u[2]), p.height_min);
+      break;
+    default: {                                    // ASE_TASK_STRIKE, humanoid_strike.py:108-128
+      const float dmax = u[0] < p.near_prob ? p.near_dist : p.dist_max;
+      const float dist = __fadd_rn(__fmul_rn(dmax - p.dist_min, u[1]), p.dist_min);
+      const float th = __fmul_rn(kTwoPi, u[2]);
+      t[0] = __fadd_rn(__fmul_rn(dist, cosf(th)), r[0]);
+      t[1] = __fadd_rn(__fmul_rn(dist, sinf(th)), r[1]);
+      t[2] = p.target_height;
+      const Quat q = quat_from_angle_axis(__fmul_rn(kTwoPi, u[3]), {0.0f, 0.0f, 1.0f});
+      t[3] = q.x; t[4] = q.y; t[5] = q.z; t[6] = q.w;
+      for (int c = 7; c < 13; ++c) t[c] = 0.0f;
+      return;                                     // the strike target has no change schedule
+    }
+  }
+  int64_t steps;
+  if (steps_in) steps = steps_in[e];
+  else steps = p.change_steps_min + (int64_t)(philox_u4(rng, (uint32_t)sid + 1u, (uint32_t)e, 0xFFFFFFFEu).x %
+                                              (uint32_t)max(1, p.change_steps_max - p.change_steps_min));
+  change_steps[e] = progress[e] + steps;
+}
+
 }  // namespace ase
 
 extern "C" int ase_policy_sample_rng(const float* mu, const float* logstd, const float* rand_probs, int rows, int act_dim, const uint64_t* rng, int stream_id,
@@ -395,6 +490,40 @@ extern "C" int ase_humanoid_reset(const int64_t* progress, const float* contact,
   ase::humanoid_reset_kernel<<<ase::ceil_div((int64_t)num_envs * 32, 256), 256, 0, (cudaStream_t)stream>>>(progress, contact, contact_env_stride, contact_body_stride, body_state,
                                                                                                          env_stride, body_stride, num_bodies, is_contact_body, termination_heights,
                                                                                                          max_episode_length, enable_early_termination, num_envs, reset_out, terminate_out);
+  ASE_LAUNCH_OK();
+  return ASE_OK;
+}
+
+extern "C" int ase_strike_reset(const int64_t* progress, const float* contact, int64_t contact_env_stride, int64_t contact_body_stride, const float* body_state,
+                                int64_t env_stride, int64_t body_stride, int num_bodies, const uint8_t* is_contact_body, const uint8_t* is_strike_body,
+                                const float* termination_heights, const float* tar_contact, int64_t tar_contact_stride, float max_episode_length,
+                                int enable_early_termination, int num_envs, uint8_t* reset_out, uint8_t* terminate_out, void* stream) {
+  ASE_CHECK_ARG(progress && reset_out && terminate_out && num_bodies > 0, "ase_strike_reset: null pointer");
+  ASE_CHECK_ARG(!enable_early_termination || (contact && body_state && is_contact_body && is_strike_body && termination_heights && tar_contact),
+                "ase_strike_reset: early termination inputs");
+  if (num_envs <= 0) return ASE_OK;
+  ase::strike_reset_kernel<<<ase::ceil_div((int64_t)num_envs * 32, 256), 256, 0, (cudaStream_t)stream>>>(
+      progress, contact, contact_env_stride, contact_body_stride, body_state, env_stride, body_stride, num_bodies, is_contact_body, is_strike_body,
+      termination_heights, tar_contact, tar_contact_stride, max_episode_length, enable_early_termination, num_envs, reset_out, terminate_out);
+  ASE_LAUNCH_OK();
+  return ASE_OK;
+}
+
+extern "C" int ase_task_resample(const AseTaskParams* p, const float* root_states, int64_t root_stride, const int64_t* progress, const uint8_t* reset_mask,
+                                 int num_envs, float* tar, int64_t tar_stride, float* tar_speed, float* tar_face_dir, int64_t* change_steps,
+                                 const uint64_t* rng, int stream_id, const float* u_in, const int64_t* steps_in, void* stream) {
+  ASE_CHECK_ARG(p && tar && (progress || (p && p->kind == ASE_TASK_STRIKE)), "ase_task_resample: null pointer");
+  ASE_CHECK_ARG(p->kind >= ASE_TASK_HEADING && p->kind <= ASE_TASK_STRIKE, "ase_task_resample: unknown task kind %d", p->kind);
+  ASE_CHECK_ARG(p->kind != ASE_TASK_STRIKE || reset_mask, "ase_task_resample: the strike target is only resampled on reset (reset_mask required)");
+  ASE_CHECK_ARG(p->kind == ASE_TASK_STRIKE || change_steps, "ase_task_resample: change_steps required");
+  ASE_CHECK_ARG(p->kind != ASE_TASK_HEADING || (tar_speed && tar_face_dir), "ase_task_resample: heading needs tar_speed and tar_face_dir");
+  ASE_CHECK_ARG(p->kind == ASE_TASK_REACH || p->kind == ASE_TASK_HEADING || root_states, "ase_task_resample: root_states required");
+  ASE_CHECK_ARG(p->kind == ASE_TASK_STRIKE || p->change_steps_max > p->change_steps_min, "ase_task_resample: empty change-steps range");
+  ASE_CHECK_ARG(rng || (u_in && (steps_in || p->kind == ASE_TASK_STRIKE)), "ase_task_resample: rng state or injected draws required");
+  if (num_envs <= 0) return ASE_OK;
+  ase::task_resample_kernel<<<ase::ceil_div(num_envs, 128), 128, 0, (cudaStream_t)stream>>>(*p, root_states, root_stride, progress, reset_mask, num_envs, tar,
+                                                                                          tar_stride, tar_speed, tar_face_dir, change_steps, rng, stream_id,
+                                                                                          u_in, steps_in);
   ASE_LAUNCH_OK();
   return ASE_OK;
 }

@@ -57,6 +57,15 @@ class GatherBatch(C.Structure):
     _fields_ = [('count', i32), ('item', GatherItem * ASE_GATHER_MAX)]
 
 
+TASK_HEADING, TASK_LOCATION, TASK_REACH, TASK_STRIKE = 0, 1, 2, 3
+
+
+class TaskParams(C.Structure):
+    _fields_ = [('kind', i32), ('change_steps_min', i32), ('change_steps_max', i32), ('speed_min', f32), ('speed_max', f32), ('rand_heading', i32),
+                ('dist_max', f32), ('height_min', f32), ('height_max', f32), ('dist_min', f32), ('near_dist', f32), ('near_prob', f32),
+                ('target_height', f32)]
+
+
 class LearnerConfig(C.Structure):
     _fields_ = [('kind', i32), ('obs_dim', i32), ('act_dim', i32), ('amp_dim', i32), ('latent_dim', i32),
                 ('n_units', i32), ('units', i32 * ASE_MAX_LAYERS),
@@ -86,7 +95,7 @@ class TrainResult(C.Structure):
 
 # every symbol declared in include/ase_b200.h (tests/test_abi.py checks the two lists agree)
 EXPORTS = ['ase_abi_version', 'ase_last_error', 'ase_launch_count', 'ase_obs_build', 'ase_amp_obs_build',
-           'ase_rms_scratch_bytes', 'ase_rms_update', 'ase_rms_apply', 'ase_gae', 'ase_amp_rewards', 'ase_heading_obs', 'ase_heading_reward', 'ase_motion_state', 'ase_amp_obs_demo', 'ase_policy_sample', 'ase_policy_sample_rng', 'ase_latent_update', 'ase_rollout_post_step', 'ase_humanoid_reset', 'ase_adv_normalize', 'ase_gather_rows',
+           'ase_rms_scratch_bytes', 'ase_rms_update', 'ase_rms_apply', 'ase_gae', 'ase_amp_rewards', 'ase_heading_obs', 'ase_heading_reward', 'ase_location_obs', 'ase_location_reward', 'ase_reach_obs', 'ase_reach_reward', 'ase_strike_obs', 'ase_strike_reward', 'ase_motion_state', 'ase_amp_obs_demo', 'ase_policy_sample', 'ase_policy_sample_rng', 'ase_latent_update', 'ase_rollout_post_step', 'ase_humanoid_reset', 'ase_strike_reset', 'ase_task_resample', 'ase_adv_normalize', 'ase_gather_rows',
            'ase_gemm', 'ase_gemm_tc_workspace_bytes', 'ase_gemm_tc_profile', 'ase_gemm_tc_profile_read', 'ase_learner_num_params', 'ase_learner_param_desc',
            'ase_learner_arena_floats', 'ase_learner_workspace_bytes', 'ase_learner_create', 'ase_learner_destroy', 'ase_learner_params_changed', 'ase_learner_plane_status', 'ase_learner_plane_flag_to', 'ase_learner_plane_flag_clear',
            'ase_learner_calc_gradients', 'ase_learner_adam_step', 'ase_learner_eval_actor_critic',
@@ -116,6 +125,12 @@ def _load():
     lib.ase_amp_rewards.argtypes = [vp, vp, vp, i32, i32, f32, f32, vp, f32, f32, f32, vp, vp, vp, vp]
     lib.ase_heading_obs.argtypes = [vp, i64, vp, vp, vp, i32, vp, i64, i32, vp]
     lib.ase_heading_reward.argtypes = [vp, i64, vp, i64, vp, i64, vp, vp, vp, f32, i32, vp, vp]
+    lib.ase_location_obs.argtypes = [vp, i64, vp, i32, vp, i64, i32, vp]
+    lib.ase_location_reward.argtypes = [vp, i64, vp, i64, vp, f32, f32, i32, vp, vp]
+    lib.ase_reach_obs.argtypes = [vp, i64, vp, i32, vp, i64, i32, vp]
+    lib.ase_reach_reward.argtypes = [vp, i64, i64, i32, vp, i32, vp, vp]
+    lib.ase_strike_obs.argtypes = [vp, i64, vp, i64, i32, vp, i64, i32, vp]
+    lib.ase_strike_reward.argtypes = [vp, i64, vp, i64, vp, i64, f32, i32, vp, vp]
     lib.ase_motion_state.argtypes = [C.POINTER(MotionLibParams), vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.ase_amp_obs_demo.argtypes = [C.POINTER(MotionLibParams), vp, vp, i32, f32, i32, i32, i32, vp, vp]
     lib.ase_policy_sample.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp, vp, vp]
@@ -124,6 +139,8 @@ def _load():
     lib.ase_latent_update.argtypes = [vp, i32, vp, vp, vp, i32, i32, i32, vp, i32, vp, vp, vp]
     lib.ase_rollout_post_step.argtypes = [vp, vp, vp, vp, vp, vp, f32, i32, vp, vp, vp, vp, vp, vp]
     lib.ase_humanoid_reset.argtypes = [vp, vp, i64, i64, vp, i64, i64, i32, vp, vp, f32, i32, i32, vp, vp, vp]
+    lib.ase_strike_reset.argtypes = [vp, vp, i64, i64, vp, i64, i64, i32, vp, vp, vp, vp, i64, f32, i32, i32, vp, vp, vp]
+    lib.ase_task_resample.argtypes = [C.POINTER(TaskParams), vp, i64, vp, vp, i32, vp, i64, vp, vp, vp, vp, i32, vp, vp, vp]
     lib.ase_learner_plane_flag_to.argtypes = [vp, vp, i32, i64, vp]
     lib.ase_learner_plane_flag_clear.argtypes = [vp, vp]
     lib.ase_gather_rows.argtypes = [C.POINTER(GatherBatch), vp]

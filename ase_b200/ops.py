@@ -208,6 +208,121 @@ def compute_heading_reward(root_pos, prev_root_pos, root_rot, tar_dir, tar_speed
     return r
 
 
+# ---- the other three HRL tasks (env/tasks/humanoid_{location,reach,strike}.py) and their target resampling -------------------------------
+TASK_OBS_SIZE = {'heading': 5, 'location': 2, 'reach': 3, 'strike': 15}
+REACH_BODY_SWORD_SHIELD = 6                       # reachBodyName: sword (humanoid_sword_shield_reach.yaml:29)
+STRIKE_BODY_IDS_SWORD_SHIELD = [6, 5, 4]          # strikeBodyNames: sword, right_hand, right_lower_arm (humanoid_sword_shield_strike.yaml:22)
+# the YAML constants of ase/data/cfg/humanoid_sword_shield_<task>.yaml and the strike task's hard-coded ones (humanoid_strike.py:19-22,117)
+TASK_PARAMS = {
+    'heading': dict(change_steps_min=100, change_steps_max=200, speed_min=1.5, speed_max=1.6, rand_heading=1),
+    'location': dict(change_steps_min=100, change_steps_max=200, dist_max=10.0),
+    'reach': dict(change_steps_min=50, change_steps_max=100, dist_max=1.0, height_min=0.2, height_max=2.0),
+    'strike': dict(dist_max=10.0, dist_min=0.5, near_dist=1.5, near_prob=0.5, target_height=0.9),
+}
+_TASK_KIND = {'heading': L.TASK_HEADING, 'location': L.TASK_LOCATION, 'reach': L.TASK_REACH, 'strike': L.TASK_STRIKE}
+
+
+def _rows(t, name):
+    if not (t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 and t.stride(1) == 1):
+        raise TypeError(f"{name}: expected CUDA float32 rows with a contiguous last dim")
+    return t.stride(0)
+
+
+def compute_location_observations(root_states, tar_pos, out=None, col0=0):
+    """env/tasks/humanoid_location.py:169-182 -> [N,2] (or written into out[:, col0:col0+2])."""
+    n = root_states.shape[0]
+    rs = _rows(root_states, 'root_states'); tar_pos = _f32c(tar_pos, 'tar_pos')
+    if out is None:
+        out = torch.empty(n, 2, device=root_states.device, dtype=torch.float32)
+    check(lib.ase_location_obs(_p(root_states), rs, _p(tar_pos), n, _p(out), out.stride(0), col0, _stream()), 'ase_location_obs')
+    return out
+
+
+def compute_location_reward(root_states, prev_root_pos, tar_pos, tar_speed, dt, out=None):
+    """env/tasks/humanoid_location.py:184-228 -> [N]."""
+    n = root_states.shape[0]
+    rs = _rows(root_states, 'root_states'); ps = _rows(prev_root_pos, 'prev_root_pos'); tar_pos = _f32c(tar_pos, 'tar_pos')
+    if out is None:
+        out = torch.empty(n, device=root_states.device, dtype=torch.float32)
+    check(lib.ase_location_reward(_p(root_states), rs, _p(prev_root_pos), ps, _p(tar_pos), float(tar_speed), float(dt), n, _p(out), _stream()),
+          'ase_location_reward')
+    return out
+
+
+def compute_reach_observations(root_states, tar_pos, out=None, col0=0):
+    """env/tasks/humanoid_reach.py:174-182 -> [N,3]: the absolute target rotated by the inverse heading."""
+    n = root_states.shape[0]
+    rs = _rows(root_states, 'root_states'); tar_pos = _f32c(tar_pos, 'tar_pos')
+    if out is None:
+        out = torch.empty(n, 3, device=root_states.device, dtype=torch.float32)
+    check(lib.ase_reach_obs(_p(root_states), rs, _p(tar_pos), n, _p(out), out.stride(0), col0, _stream()), 'ase_reach_obs')
+    return out
+
+
+def compute_reach_reward(body_state, tar_pos, reach_body=REACH_BODY_SWORD_SHIELD, out=None):
+    """env/tasks/humanoid_reach.py:184-195 on the rigid-body state [N, J, 13] -> [N]."""
+    n = body_state.shape[0]
+    es, bs = _body_strides(body_state); tar_pos = _f32c(tar_pos, 'tar_pos')
+    if out is None:
+        out = torch.empty(n, device=body_state.device, dtype=torch.float32)
+    check(lib.ase_reach_reward(_p(body_state), es, bs, int(reach_body), _p(tar_pos), n, _p(out), _stream()), 'ase_reach_reward')
+    return out
+
+
+def compute_strike_observations(root_states, tar_states, out=None, col0=0):
+    """env/tasks/humanoid_strike.py:193-216 -> [N,15]."""
+    n = root_states.shape[0]
+    rs = _rows(root_states, 'root_states'); ts = _rows(tar_states, 'tar_states')
+    if out is None:
+        out = torch.empty(n, 15, device=root_states.device, dtype=torch.float32)
+    check(lib.ase_strike_obs(_p(root_states), rs, _p(tar_states), ts, n, _p(out), out.stride(0), col0, _stream()), 'ase_strike_obs')
+    return out
+
+
+def compute_strike_reward(tar_states, root_states, prev_root_pos, dt, out=None):
+    """env/tasks/humanoid_strike.py:218-251 -> [N]."""
+    n = root_states.shape[0]
+    ts = _rows(tar_states, 'tar_states'); rs = _rows(root_states, 'root_states'); ps = _rows(prev_root_pos, 'prev_root_pos')
+    if out is None:
+        out = torch.empty(n, device=root_states.device, dtype=torch.float32)
+    check(lib.ase_strike_reward(_p(tar_states), ts, _p(root_states), rs, _p(prev_root_pos), ps, float(dt), n, _p(out), _stream()), 'ase_strike_reward')
+    return out
+
+
+def compute_strike_reset(progress_buf, contact_buf, is_contact_body, is_strike_body, body_state, tar_contact_forces, max_episode_length,
+                         enable_early_termination, termination_heights, reset_out=None, terminate_out=None):
+    """env/tasks/humanoid_strike.py:254-295 -> (reset, terminated) uint8 [N].  contact_buf [N, J, 3]; tar_contact_forces [N, 3] rows;
+    is_contact_body / is_strike_body uint8 [J]."""
+    n, j, _ = body_state.shape
+    es, bs = _body_strides(body_state)
+    if reset_out is None:
+        reset_out = torch.empty(n, dtype=torch.uint8, device=body_state.device)
+    if terminate_out is None:
+        terminate_out = torch.empty(n, dtype=torch.uint8, device=body_state.device)
+    assert contact_buf.stride(2) == 1 and tar_contact_forces.stride(1) == 1
+    check(lib.ase_strike_reset(_p(progress_buf), _p(contact_buf), contact_buf.stride(0), contact_buf.stride(1), _p(body_state), es, bs, j,
+                               _p(is_contact_body), _p(is_strike_body), _p(termination_heights), _p(tar_contact_forces), tar_contact_forces.stride(0),
+                               float(max_episode_length), int(bool(enable_early_termination)), n, _p(reset_out), _p(terminate_out), _stream()),
+          'ase_strike_reset')
+    return reset_out, terminate_out
+
+
+def task_resample(task, tar, progress, root_states=None, reset_mask=None, tar_speed=None, tar_face_dir=None, change_steps=None, rng=None,
+                  stream_id=0, u_in=None, steps_in=None, params=None):
+    """_update_task (reset_mask None: envs with progress >= change_steps) / _reset_task / strike _reset_target (envs flagged in the uint8
+    reset_mask) without nonzero().  tar: heading tar_dir [N,2], location tar_pos [N,2], reach tar_pos [N,3], strike target states [N,13] rows.
+    params overrides entries of TASK_PARAMS[task].  Draws come from the Philox stream {rng, stream_id} or from u_in [N,4] / steps_in [N]."""
+    kw = dict(TASK_PARAMS[task], **(params or {}))
+    p = L.TaskParams(kind=_TASK_KIND[task], **kw)
+    n = tar.shape[0]
+    ts = _rows(tar, 'tar')
+    rs = 0 if root_states is None else _rows(root_states, 'root_states')
+    assert change_steps is None or change_steps.dtype == torch.int64
+    assert progress is None or progress.dtype == torch.int64
+    check(lib.ase_task_resample(C.byref(p), _p(root_states), rs, _p(progress), _p(reset_mask), n, _p(tar), ts, _p(tar_speed), _p(tar_face_dir),
+                                _p(change_steps), _p(rng), int(stream_id), _p(u_in), _p(steps_in), _stream()), 'ase_task_resample')
+
+
 def policy_sample(mu, logstd, noise, rand_mask=None):
     """Eval-mode Gaussian head + eps-greedy override (amp_agent.py:139-169) -> (actions, neglogpacs, sigmas)."""
     rows, a = mu.shape

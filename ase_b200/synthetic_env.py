@@ -6,7 +6,12 @@ history, resets -- runs through the CUDA kernels exactly as post_physics_step wo
 
 `state_source`:
   'device' : a pool of pre-generated states resident in HBM (bench `value`)
-  'host'   : states arrive from PINNED HOST memory every step (bench `e2e`; H2D copy inside the step)"""
+  'host'   : states arrive from PINNED HOST memory every step (bench `e2e`; H2D copy inside the step)
+
+`task` (HumanoidHeading / HumanoidLocation / HumanoidReach / HumanoidStrike, env/tasks/humanoid_<task>.py): the task observation is
+appended behind the humanoid features, the task reward replaces the zero reward, and targets are resampled on the device the way
+_update_task / _reset_task / _reset_target do, with in-kernel Philox draws (no host sync, CUDA-graph capturable).  `heading_task=True` is
+the older heading stand-in with FIXED targets (no resampling) and stays as it was."""
 import numpy as np
 import torch
 
@@ -33,17 +38,24 @@ class SyntheticHumanoidEnv:
     NUM_BODIES, NUM_DOFS, AMP_STEPS, AMP_STEP_DIM = 17, 31, 10, 140
 
     def __init__(self, num_envs, device='cuda', seed=0, pool=8, state_source='device', done_prob=1.0 / 300.0,
-                 local_root_obs=True, root_height_obs=True, demo_pool=8192, heading_task=False, dt=1.0 / 30.0, demo_source='motion_lib'):
+                 local_root_obs=True, root_height_obs=True, demo_pool=8192, heading_task=False, dt=1.0 / 30.0, demo_source='motion_lib',
+                 task=None):
+        if task is not None and heading_task:
+            raise ValueError("heading_task=True (fixed targets) and task=... (resampled targets) exclude each other")
+        if task is not None and task not in ops.TASK_OBS_SIZE:
+            raise ValueError(f"task must be one of {sorted(ops.TASK_OBS_SIZE)}, got {task!r}")
         self.device = torch.device(device)
+        self.task_name = task
         self.num_envs = num_envs
         self.local_root_obs, self.root_height_obs = local_root_obs, root_height_obs
         self.state_source = state_source
         self.done_prob = done_prob
         self.heading_task, self.dt = heading_task, dt
-        self.task = _Task(num_envs, self.device, 5 if heading_task else 0)     # HumanoidHeading: 5 task-obs floats
+        task_obs = 5 if heading_task else (ops.TASK_OBS_SIZE[task] if task else 0)      # HumanoidHeading: 5 task-obs floats
+        self.task = _Task(num_envs, self.device, task_obs)
         self.env = self                      # agents reach vec_env.env.task / vec_env.env.fetch_amp_obs_demo
         self.num_humanoid_obs = 1 + 16 * 3 + 17 * 6 + 17 * 3 + 17 * 3
-        self.num_obs = self.num_humanoid_obs + (5 if heading_task else 0)
+        self.num_obs = self.num_humanoid_obs + task_obs
         self.num_amp_obs = self.AMP_STEPS * self.AMP_STEP_DIM
         self.observation_space = _Box(-np.inf * np.ones(self.num_obs), np.inf * np.ones(self.num_obs))
         self.amp_observation_space = _Box(-np.inf * np.ones(self.num_amp_obs), np.inf * np.ones(self.num_amp_obs))
@@ -96,9 +108,13 @@ class SyntheticHumanoidEnv:
             self._tar_face_dir = torch.stack([torch.cos(fh), torch.sin(fh)], dim=-1).to(self.device)
             self._tar_speed = (1.0 + 4.0 * torch.rand(num_envs, generator=g)).to(self.device)
             self._prev_root_pos = torch.zeros(num_envs, 3, device=self.device)
+        if task is not None:
+            self._init_task(seed)
         self._load_state()
-        if heading_task:
+        if heading_task or task is not None:
             self._prev_root_pos.copy_(self._body[:, 0, 0:3])
+        if task is not None:      # every env starts with a sampled target (HumanoidAMPTask._reset_envs -> _reset_task at the first reset)
+            self._resample_task(self._all_envs)
         self._compute_observations(shift=False)
         self._amp_obs_buf[:, 1:] = self._amp_obs_buf[:, 0:1]
 
@@ -144,19 +160,27 @@ class SyntheticHumanoidEnv:
         if self.heading_task:      # humanoid_amp_task.py:51-64: task obs appended behind the humanoid features
             ops.compute_heading_observations(self._body[:, 0], self._tar_dir, self._tar_speed, self._tar_face_dir, out=self.obs_buf,
                                              col0=self.num_humanoid_obs)
+        elif self.task_name is not None:
+            self._compute_task_obs()
         ops.build_amp_observations(self._body, self._dof[:, :D], self._dof[:, D:], self._amp_obs_buf, self.local_root_obs,
                                    self.root_height_obs, shift_history=shift, env_ids=env_ids, env_mask=env_mask, fill_history=fill_history)
 
     def step(self, actions):
-        """base_task.py:119-137: physics (bypassed: next synthetic state) then post_physics_step."""
-        if self.heading_task:
+        """base_task.py:119-137: pre_physics_step (prev_root_pos; _update_task), physics (bypassed: next synthetic state), then
+        post_physics_step."""
+        if self.heading_task or self.task_name is not None:
             self._prev_root_pos.copy_(self._body[:, 0, 0:3])
+        if self.task_name is not None and self.task_name != 'strike':
+            self._resample_task(None)                       # _update_task: envs with progress >= change_steps
         self._load_state()
         self.task.progress_buf += 1
         self._compute_observations(shift=True)
         if self.heading_task:
             self.rew_buf = ops.compute_heading_reward(self._body[:, 0, 0:3], self._prev_root_pos, self._body[:, 0, 3:7], self._tar_dir,
                                                       self._tar_speed, self._tar_face_dir, self.dt)
+        elif self.task_name is not None:
+            self._compute_task_reward()
+            self._task_rng[1:].add_(1)                      # every task draw of this step has been taken (a launch of its own)
         # (the default CUDA generator: it is CUDA-graph safe, a private torch.Generator is not)
         r = torch.rand(self.num_envs, device=self.device) if self.device.type == 'cuda' else torch.rand(self.num_envs, generator=self._gen)
         torch.lt(r, self.done_prob, out=self._done_bool); torch.lt(r, 0.5 * self.done_prob, out=self._term_bool)
@@ -174,15 +198,78 @@ class SyntheticHumanoidEnv:
         if len(env_ids) > 0:
             ids = env_ids.to(torch.int32)
             self.task.progress_buf[env_ids] = 0
+            mask = None
+            if self.task_name is not None:
+                mask = torch.zeros(self.num_envs, dtype=torch.uint8, device=self.device); mask[env_ids] = 1
+            if self.task_name == 'strike':
+                self._resample_task(mask)
             self._compute_observations(shift=False, env_ids=ids)
             self._amp_obs_buf[env_ids, 1:] = self._amp_obs_buf[env_ids, 0:1]
+            if self.task_name is not None and self.task_name != 'strike':
+                self._resample_task(mask)
         return self.obs_buf
 
     def reset_done(self, mask):
         """The same reset driven by a uint8 [N] mask on the device: no index list, no host sync (the agents use it when the env offers it)."""
         self.task.progress_buf.masked_fill_(mask.bool(), 0)
+        if self.task_name == 'strike':            # _reset_target runs inside _reset_actors, before the observation is built
+            self._resample_task(mask)
         self._compute_observations(shift=False, env_mask=mask, fill_history=True)
+        if self.task_name is not None and self.task_name != 'strike':
+            self._resample_task(mask)             # HumanoidAMPTask._reset_envs: _reset_task after the observation (it carries the old target)
         return self.obs_buf
+
+    # ---- the location / reach / strike tasks and device-side resampling for all four (task=...) ------------------------------------
+    def _init_task(self, seed):
+        n, dev = self.num_envs, self.device
+        self._prev_root_pos = torch.zeros(n, 3, device=dev)
+        self._tar_change_steps = torch.zeros(n, dtype=torch.int64, device=dev)
+        self._all_envs = torch.ones(n, dtype=torch.uint8, device=dev)
+        self._task_rng = torch.tensor([seed * 7919 + 104729, 0], dtype=torch.int64, device=dev)     # {seed, step counter} of the Philox stream
+        t = self.task_name
+        if t == 'heading':
+            self._tar_dir = torch.zeros(n, 2, device=dev); self._tar_dir[:, 0] = 1.0
+            self._tar_face_dir = self._tar_dir.clone()
+            self._tar_speed = torch.ones(n, device=dev)
+        elif t == 'location':
+            self._tar_pos = torch.zeros(n, 2, device=dev)
+        elif t == 'reach':
+            self._tar_pos = torch.zeros(n, 3, device=dev)
+        else:
+            self._tar_states = torch.zeros(n, 13, device=dev)
+
+    def _resample_task(self, mask):
+        """mask None: update mode (_update_task); a uint8 [N] mask: reset mode for the flagged envs.  Update and reset draw from different
+        Philox streams, so a step's two calls never share draws."""
+        t = self.task_name
+        tar = {'heading': getattr(self, '_tar_dir', None), 'strike': getattr(self, '_tar_states', None)}.get(t, getattr(self, '_tar_pos', None))
+        ops.task_resample(t, tar, self.task.progress_buf, root_states=self._body[:, 0], reset_mask=mask,
+                          tar_speed=getattr(self, '_tar_speed', None) if t == 'heading' else None,
+                          tar_face_dir=getattr(self, '_tar_face_dir', None) if t == 'heading' else None,
+                          change_steps=None if t == 'strike' else self._tar_change_steps, rng=self._task_rng, stream_id=0 if mask is None else 2)
+
+    def _compute_task_obs(self):
+        root, col0, t = self._body[:, 0], self.num_humanoid_obs, self.task_name
+        if t == 'heading':
+            ops.compute_heading_observations(root, self._tar_dir, self._tar_speed, self._tar_face_dir, out=self.obs_buf, col0=col0)
+        elif t == 'location':
+            ops.compute_location_observations(root, self._tar_pos, out=self.obs_buf, col0=col0)
+        elif t == 'reach':
+            ops.compute_reach_observations(root, self._tar_pos, out=self.obs_buf, col0=col0)
+        else:
+            ops.compute_strike_observations(root, self._tar_states, out=self.obs_buf, col0=col0)
+
+    def _compute_task_reward(self):
+        root, t = self._body[:, 0], self.task_name
+        if t == 'heading':
+            self.rew_buf = ops.compute_heading_reward(root[:, 0:3], self._prev_root_pos, root[:, 3:7], self._tar_dir, self._tar_speed,
+                                                      self._tar_face_dir, self.dt)
+        elif t == 'location':
+            ops.compute_location_reward(root, self._prev_root_pos, self._tar_pos, 1.0, self.dt, out=self.rew_buf)      # tarSpeed: 1.0
+        elif t == 'reach':
+            ops.compute_reach_reward(self._body, self._tar_pos, out=self.rew_buf)
+        else:
+            ops.compute_strike_reward(self._tar_states, root, self._prev_root_pos, self.dt, out=self.rew_buf)
 
     def on_graph_replay(self, steps):
         """A captured rollout was replayed: advance the host-side step counter the capture baked in (the pool index pattern repeats

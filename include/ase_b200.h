@@ -141,6 +141,28 @@ int ase_heading_reward(const float* root_pos, int64_t root_pos_stride, const flo
                        const float* root_rot, int64_t rot_stride, const float* tar_dir, const float* tar_speed,
                        const float* tar_face_dir, float dt, int num_envs, float* reward, void* stream);
 
+/* HRL location / reach / strike tasks (the other three shipped high-level controllers).  Same conventions as the heading task: root_states and
+ * tar_states are [N, 13] rows with an explicit stride (26 when both are views of Isaac Gym's _root_states with 2 actors per env), task obs are
+ * written at obs + obs_col0 with row stride obs_ld.
+ *   ase_location_obs    compute_location_observations  env/tasks/humanoid_location.py:169-182   tar_pos [N,2] (z = 0) -> 2 floats
+ *   ase_location_reward compute_location_reward        env/tasks/humanoid_location.py:184-228   prev_root_pos [N,3] rows with prev_stride
+ *   ase_reach_obs       compute_location_observations  env/tasks/humanoid_reach.py:174-182      tar_pos [N,3], absolute (not root-relative) -> 3
+ *   ase_reach_reward    compute_reach_reward           env/tasks/humanoid_reach.py:184-195      reach body `reach_body` of the [N,J,13] rigid-body state
+ *   ase_strike_obs      compute_strike_observations    env/tasks/humanoid_strike.py:193-216     -> 15 floats
+ *   ase_strike_reward   compute_strike_reward          env/tasks/humanoid_strike.py:218-251     (strike_body_vel / near_dist are unused there) */
+int ase_location_obs(const float* root_states, int64_t root_stride, const float* tar_pos, int num_envs, float* obs, int64_t obs_ld, int obs_col0,
+                     void* stream);
+int ase_location_reward(const float* root_states, int64_t root_stride, const float* prev_root_pos, int64_t prev_stride, const float* tar_pos,
+                        float tar_speed, float dt, int num_envs, float* reward, void* stream);
+int ase_reach_obs(const float* root_states, int64_t root_stride, const float* tar_pos, int num_envs, float* obs, int64_t obs_ld, int obs_col0,
+                  void* stream);
+int ase_reach_reward(const float* body_state, int64_t env_stride, int64_t body_stride, int reach_body, const float* tar_pos, int num_envs,
+                     float* reward, void* stream);
+int ase_strike_obs(const float* root_states, int64_t root_stride, const float* tar_states, int64_t tar_stride, int num_envs, float* obs,
+                   int64_t obs_ld, int obs_col0, void* stream);
+int ase_strike_reward(const float* tar_states, int64_t tar_stride, const float* root_states, int64_t root_stride, const float* prev_root_pos,
+                      int64_t prev_stride, float dt, int num_envs, float* reward, void* stream);
+
 /* Gaussian head in eval mode (rl_games ModelA2CContinuousLogStd.forward, is_train False) + the eps-greedy
  * override of get_action_values (amp_agent.py:164-167): a = mu + exp(logstd)*noise, neglogp(a); rows whose
  * rand_mask is 0 act deterministically (a := mu) but keep the sampled action's neglogp, as the reference does.
@@ -174,6 +196,37 @@ int ase_humanoid_reset(const int64_t* progress, const float* contact, int64_t co
                        const float* body_state, int64_t env_stride, int64_t body_stride, int num_bodies, const uint8_t* is_contact_body,
                        const float* termination_heights, float max_episode_length, int enable_early_termination, int num_envs,
                        uint8_t* reset_out, uint8_t* terminate_out, void* stream);
+/* compute_humanoid_reset of the strike task, env/tasks/humanoid_strike.py:254-295: the base rule above, plus failure when the target's contact
+ * force tar_contact [N,3] (rows with tar_contact_stride: body num_bodies of the net-contact tensor) exceeds 1.0 in x or y while a body that is
+ * neither a contact body nor a strike body (is_strike_body [J]: sword, right_hand, right_lower_arm) has a force component above 1.0. */
+int ase_strike_reset(const int64_t* progress, const float* contact, int64_t contact_env_stride, int64_t contact_body_stride,
+                     const float* body_state, int64_t env_stride, int64_t body_stride, int num_bodies, const uint8_t* is_contact_body,
+                     const uint8_t* is_strike_body, const float* termination_heights, const float* tar_contact, int64_t tar_contact_stride,
+                     float max_episode_length, int enable_early_termination, int num_envs, uint8_t* reset_out, uint8_t* terminate_out, void* stream);
+
+/* Task target resampling without host syncs: _update_task / _reset_task of env/tasks/humanoid_heading.py:147-174,
+ * humanoid_location.py:107-125, humanoid_reach.py:111-130 and _reset_target of humanoid_strike.py:108-128.  The reference turns
+ * `progress_buf >= change_steps` into an index list with nonzero() on every pre_physics_step; here one kernel is driven by a mask.
+ *   reset_mask NULL (update mode): envs with progress >= change_steps resample (heading, location, reach; strike has no update);
+ *   reset_mask [N] uint8 (reset mode): the flagged envs resample (progress is expected to be 0 already, as after _reset_env_tensors).
+ * Targets: heading tar = tar_dir [N,2] (+ tar_speed [N], tar_face_dir [N,2]); location tar_pos [N,2]; reach tar_pos [N,3]; strike the [N,13]
+ * target state.  tar rows are tar_stride floats apart.  change_steps [N] int64 := progress + randint(min, max) (not for strike).
+ * Draws: rng / stream_id as ase_latent_update (streams stream_id and stream_id + 1; the caller advances rng[1] in a later launch), or injected
+ * u_in [N,4] (uniform k of an env is its k-th draw in the reference's order) and steps_in [N] int64. */
+typedef enum { ASE_TASK_HEADING = 0, ASE_TASK_LOCATION = 1, ASE_TASK_REACH = 2, ASE_TASK_STRIKE = 3 } AseTaskKind;
+typedef struct {
+  int kind;                                /* AseTaskKind */
+  int change_steps_min, change_steps_max;  /* heading: headingChangeSteps{Min,Max}; location / reach: tarChangeSteps{Min,Max} */
+  float speed_min, speed_max;              /* heading: tarSpeed{Min,Max} */
+  int rand_heading;                        /* heading: enableRandHeading (0: both angles 0 and the speed is the first draw) */
+  float dist_max;                          /* location / reach: tarDistMax; strike: far distance (10) */
+  float height_min, height_max;            /* reach: tarHeight{Min,Max} */
+  float dist_min, near_dist, near_prob;    /* strike: 0.5, 1.5, 0.5 */
+  float target_height;                     /* strike: 0.9 */
+} AseTaskParams;
+int ase_task_resample(const AseTaskParams* p, const float* root_states, int64_t root_stride, const int64_t* progress, const uint8_t* reset_mask,
+                      int num_envs, float* tar, int64_t tar_stride, float* tar_speed, float* tar_face_dir, int64_t* change_steps,
+                      const uint64_t* rng, int stream_id, const float* u_in, const int64_t* steps_in, void* stream);
 
 /* _calc_advs amp_agent.py:551-561 (+ torch_ext.normalization_with_masks); mask NULL => plain
  * mean / unbiased std (common_agent.py:536-546).  scratch >= 64 bytes. */
