@@ -217,7 +217,11 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
   }
   return c;
 }
-__device__ __forceinline__ float u01(uint32_t x) { return ((float)(x >> 8) + 0.5f) * (1.0f / 16777216.0f); }   // (0, 1)
+// (0, 1]: from 2^23 up, code + 0.5 rounds to an even integer, and the top code 0xFFFFFF rounds to 2^24, i.e. 1.0.  Box-Muller input only
+// (-2 log(1) = 0 is a valid radius).
+__device__ __forceinline__ float u01(uint32_t x) { return ((float)(x >> 8) + 0.5f) * (1.0f / 16777216.0f); }
+// (0, 1) like torch.rand: u01 capped at the largest float below 1, so `u < p` holds for p = 1 and a target never reaches the top of its range.
+__device__ __forceinline__ float u01_open(uint32_t x) { return fminf(u01(x), 0x1.fffffep-1f); }
 // 4 standard normals of draw `call`, stream `sid`, element group (row, grp)
 __device__ __forceinline__ float4 philox_normal4(const uint64_t* rng, uint32_t sid, uint32_t row, uint32_t grp) {
   const uint64_t seed = rng[0], call = rng[1];
@@ -241,7 +245,7 @@ policy_sample_rng_kernel(const float* __restrict__ mu, const float* __restrict__
   if (row >= rows) return;
   float m = 1.0f;                                  // rand_action_mask: bernoulli(p) (amp_agent.py:164); 1 when there is no eps-greedy
   if (mask_in) m = mask_in[row];
-  else if (rand_probs) m = (u01(philox_u4(rng, (uint32_t)sid + 1u, (uint32_t)row, 0xFFFFFFFFu).x) < rand_probs[row]) ? 1.0f : 0.0f;
+  else if (rand_probs) m = (u01_open(philox_u4(rng, (uint32_t)sid + 1u, (uint32_t)row, 0xFFFFFFFFu).x) < rand_probs[row]) ? 1.0f : 0.0f;
   const bool det = m == 0.0f;
   float s = 0.0f, sumlog = 0.0f;
   for (int j0 = lane * 4; j0 < A; j0 += 128) {
@@ -399,7 +403,7 @@ task_resample_kernel(AseTaskParams p, const float* __restrict__ root, int64_t rs
     for (int q = 0; q < 4; ++q) u[q] = u_in[(int64_t)e * 4 + q];
   } else {
     const uint4 r = philox_u4(rng, (uint32_t)sid, (uint32_t)e, 0u);
-    u[0] = u01(r.x); u[1] = u01(r.y); u[2] = u01(r.z); u[3] = u01(r.w);
+    u[0] = u01_open(r.x); u[1] = u01_open(r.y); u[2] = u01_open(r.z); u[3] = u01_open(r.w);
   }
   const float kTwoPi = 6.28318530717958647692f, kPi = 3.14159265358979323846f;
   const float* r = root + (int64_t)e * rs;

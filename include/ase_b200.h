@@ -174,7 +174,14 @@ int ase_policy_sample(const float* mu, const float* logstd, const float* noise, 
  * `_latent_reset_steps <= progress_buf` into index lists with nonzero() (a host sync per sim step).  These entry points run the same
  * arithmetic mask-driven, with a counter-based generator (Philox4x32-10) evaluated inside the kernels: `rng` is a 2-element device array
  * {seed, call counter}; ase_rollout_post_step advances the counter, so a whole rollout can be captured in a CUDA graph.  Each takes
- * optional injected draws (parity tests feed the reference's own draws). */
+ * optional injected draws (parity tests feed the reference's own draws).
+ * Addressing: rng is read as uint64 (negative seeds wrap).  Words (x, y, z, w) of block (row, group) of stream sid are
+ * Philox4x32-10(counter = (row, group, call lo, call hi), key = (seed lo, seed hi ^ sid * 0x9E3779B1)).  A 32-bit word x becomes
+ * u = (fp32(x >> 8) + 0.5f) * 2^-24 in (0, 1] (the top code rounds to 1.0); Box-Muller normals (stream sid, group = column / 4,
+ * (a cos, a sin, b cos, b sin) with radii from x and z, angles from y and w) take u as it is.  The Bernoulli draw (stream sid + 1, group
+ * 0xFFFFFFFF, word x: u < p) and the task uniforms (stream sid, group 0, words x..w) take min(u, 1 - 2^-24), in (0, 1) like torch.rand,
+ * so p = 1 always gives 1 and a target never reaches the top of its range.  Randints (stream sid + 1, group 0xFFFFFFFE, word x) are
+ * min + x % max(1, max - min).  oracle/philox_oracle.py restates all of it. */
 /* get_action_values' sampling half (rl_games ModelA2CContinuousLogStd eval + amp_agent.py:164-167): a = mu + exp(logstd) * noise,
  * rand_action_mask = bernoulli(rand_probs) (all ones when rand_probs is NULL), masked rows act deterministically. */
 int ase_policy_sample_rng(const float* mu, const float* logstd, const float* rand_probs, int rows, int act_dim,

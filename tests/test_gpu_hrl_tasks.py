@@ -178,7 +178,8 @@ def test_task_resample_philox_ranges_determinism_and_graph(task):
         d = tar - root[:, 0:2]
         assert float(d.abs().max()) <= P['dist_max'] * (1 + 1e-6)
     elif task == 'reach':
-        assert float(tar[:, 0:2].abs().max()) <= P['dist_max'] and float(tar[:, 2].min()) >= 0.2 and float(tar[:, 2].max()) <= 2.0
+        assert float(tar[:, 0:2].abs().max()) < P['dist_max'] and float(tar[:, 2].min()) >= P['height_min']
+        assert float(tar[:, 2].max()) < P['height_max']                # [min, max) like torch.rand
     else:
         dist = (tar[:, 0:2] - root[:, 0:2]).norm(dim=-1)
         assert float(dist.min()) >= 0.5 - 1e-4 and float(dist.max()) <= 10.0 + 1e-4

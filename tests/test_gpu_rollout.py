@@ -154,10 +154,8 @@ def _tables(fx, seed):
                 steps=torch.randint(1, 6, (H, N), generator=g, dtype=torch.int32).cuda())
 
 
-def test_device_rollout_equals_reference_order_rollout_and_never_syncs():
-    fx = G.load('rollout_ase.pt')
-    tb = _tables(fx, 5)
-    # (a) reference-order rollout drawing from per-env tables
+def reference_order_rollout(fx, tb):
+    """The reference-order rollout drawing from the per-env tables tb (noise / mask / z / steps, each [H, N, ...]) -> (agent, env)."""
     env_a = ScriptedEnv(fx)
     a = _agent(fx, env_a, device_rollout=False)
     step = {'n': -1}
@@ -179,6 +177,14 @@ def test_device_rollout_equals_reference_order_rollout_and_never_syncs():
     a.obs = {'obs': env_a.cur}
     with torch.no_grad():
         a.play_steps()
+    return a, env_a
+
+
+def test_device_rollout_equals_reference_order_rollout_and_never_syncs():
+    fx = G.load('rollout_ase.pt')
+    tb = _tables(fx, 5)
+    # (a) reference-order rollout drawing from per-env tables
+    a, env_a = reference_order_rollout(fx, tb)
     # (b) device rollout with the same tables injected into the kernels
     env_b = ScriptedEnv(fx, masked=True)
     b = _agent(fx, env_b, device_rollout=True, rollout_graph=False)
