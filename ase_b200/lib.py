@@ -66,6 +66,21 @@ class TaskParams(C.Structure):
                 ('target_height', f32)]
 
 
+STATE_INIT = {'Default': 0, 'Start': 1, 'Random': 2, 'Hybrid': 3}                      # AseStateInit (HumanoidAMP.StateInit)
+INIT_NONE, INIT_DEFAULT, INIT_REF, INIT_FALL, INIT_RECOVERY = 0, 1, 2, 3, 4            # AseInitKind
+
+
+class StateInitParams(C.Structure):
+    _fields_ = [('state_init', i32), ('hybrid_prob', f32), ('recovery_prob', f32), ('fall_prob', f32), ('recovery_steps', i32),
+                ('reset_mask', vp), ('num_envs', i32), ('root_states', vp), ('root_stride', i64),
+                ('dof_pos', vp), ('dof_pos_stride', i64), ('dof_pos_elem_stride', i64), ('dof_vel', vp), ('dof_vel_stride', i64),
+                ('dof_vel_elem_stride', i64), ('init_root_states', vp), ('init_dof_pos', vp), ('init_dof_vel', vp),
+                ('fall_root_states', vp), ('fall_dof_pos', vp), ('fall_dof_vel', vp), ('num_fall_states', i32),
+                ('recovery_counter', vp), ('progress', vp), ('reset_buf', vp), ('terminate_buf', vp),
+                ('kind_out', vp), ('motion_id_out', vp), ('motion_time_out', vp), ('rng', vp), ('stream_id', i32),
+                ('recovery_in', vp), ('fall_in', vp), ('hybrid_in', vp), ('motion_id_in', vp), ('phase_in', vp), ('fall_row_in', vp)]
+
+
 class LearnerConfig(C.Structure):
     _fields_ = [('kind', i32), ('obs_dim', i32), ('act_dim', i32), ('amp_dim', i32), ('latent_dim', i32),
                 ('n_units', i32), ('units', i32 * ASE_MAX_LAYERS),
@@ -95,7 +110,7 @@ class TrainResult(C.Structure):
 
 # every symbol declared in include/ase_b200.h (tests/test_abi.py checks the two lists agree)
 EXPORTS = ['ase_abi_version', 'ase_last_error', 'ase_launch_count', 'ase_obs_build', 'ase_amp_obs_build',
-           'ase_rms_scratch_bytes', 'ase_rms_update', 'ase_rms_apply', 'ase_gae', 'ase_amp_rewards', 'ase_heading_obs', 'ase_heading_reward', 'ase_location_obs', 'ase_location_reward', 'ase_reach_obs', 'ase_reach_reward', 'ase_strike_obs', 'ase_strike_reward', 'ase_motion_state', 'ase_amp_obs_demo', 'ase_policy_sample', 'ase_policy_sample_rng', 'ase_latent_update', 'ase_rollout_post_step', 'ase_humanoid_reset', 'ase_strike_reset', 'ase_task_resample', 'ase_adv_normalize', 'ase_gather_rows',
+           'ase_rms_scratch_bytes', 'ase_rms_update', 'ase_rms_apply', 'ase_gae', 'ase_amp_rewards', 'ase_heading_obs', 'ase_heading_reward', 'ase_location_obs', 'ase_location_reward', 'ase_reach_obs', 'ase_reach_reward', 'ase_strike_obs', 'ase_strike_reward', 'ase_motion_state', 'ase_amp_obs_demo', 'ase_policy_sample', 'ase_policy_sample_rng', 'ase_latent_update', 'ase_rollout_post_step', 'ase_humanoid_reset', 'ase_strike_reset', 'ase_task_resample', 'ase_amp_state_init', 'ase_amp_history_init', 'ase_recovery_step', 'ase_adv_normalize', 'ase_gather_rows',
            'ase_gemm', 'ase_gemm_tc_workspace_bytes', 'ase_gemm_tc_profile', 'ase_gemm_tc_profile_read', 'ase_learner_num_params', 'ase_learner_param_desc',
            'ase_learner_arena_floats', 'ase_learner_workspace_bytes', 'ase_learner_create', 'ase_learner_destroy', 'ase_learner_params_changed', 'ase_learner_plane_status', 'ase_learner_plane_flag_to', 'ase_learner_plane_flag_clear',
            'ase_learner_calc_gradients', 'ase_learner_adam_step', 'ase_learner_eval_actor_critic',
@@ -141,6 +156,9 @@ def _load():
     lib.ase_humanoid_reset.argtypes = [vp, vp, i64, i64, vp, i64, i64, i32, vp, vp, f32, i32, i32, vp, vp, vp]
     lib.ase_strike_reset.argtypes = [vp, vp, i64, i64, vp, i64, i64, i32, vp, vp, vp, vp, i64, f32, i32, i32, vp, vp, vp]
     lib.ase_task_resample.argtypes = [C.POINTER(TaskParams), vp, i64, vp, vp, i32, vp, i64, vp, vp, vp, vp, i32, vp, vp, vp]
+    lib.ase_amp_state_init.argtypes = [C.POINTER(MotionLibParams), vp, i32, C.POINTER(StateInitParams), vp]
+    lib.ase_amp_history_init.argtypes = [C.POINTER(MotionLibParams), vp, vp, vp, i32, f32, i32, i32, vp, i32, vp]
+    lib.ase_recovery_step.argtypes = [vp, vp, vp, i32, vp]
     lib.ase_learner_plane_flag_to.argtypes = [vp, vp, i32, i64, vp]
     lib.ase_learner_plane_flag_clear.argtypes = [vp, vp]
     lib.ase_gather_rows.argtypes = [C.POINTER(GatherBatch), vp]

@@ -26,6 +26,11 @@ class MotionLib:
         self.length_starts = shifted.cumsum(0).to(torch.int32).contiguous()
         w = torch.ones(len(motion_lengths)) if motion_weights is None else motion_weights
         self._motion_weights = (w / w.sum()).to(dev, torch.float32)
+        # inverse-CDF table of the device resets (ase_amp_state_init): fp32 cumsum of the normalised weights, computed in fp64, last entry 1
+        w64 = w.to(torch.float64)
+        cdf = (w64 / w64.sum()).cumsum(0)
+        cdf[-1] = 1.0
+        self._motion_cdf = cdf.to(dev, torch.float32).contiguous()
         self.device = dev
         self._num_bodies, self._num_dof = self.gts.shape[1], dof_offsets[-1]
         self._nj, self._nk = len(dof_body_ids), len(key_body_ids)

@@ -385,3 +385,59 @@ def gemm(A, B, a_trans=False, b_trans=False, bias=None, act=0, mask_src=None, ma
                      _p(mask_bits), 0 if mask_bits is None else mask_bits.stride(0), 0)
     check(lib.ase_gemm(C.byref(p), _stream()), 'ase_gemm')
     return out
+
+
+# ---- episode resets of HumanoidAMP / HumanoidAMPGetup (env/tasks/humanoid_amp.py:141-246, humanoid_amp_getup.py) -----------------------
+# the YAML constants: humanoid_ase_sword_shield_getup.yaml (ASE pre-training) and humanoid_sword_shield.yaml (AMP)
+STATE_INIT_PARAMS = {
+    'getup': dict(state_init='Hybrid', hybrid_prob=0.5, recovery_prob=0.2, recovery_steps=60, fall_prob=0.1),
+    'amp': dict(state_init='Random', hybrid_prob=0.5, recovery_prob=0.0, recovery_steps=0, fall_prob=0.0),
+}
+
+
+def _dof_strides(t, name):
+    if not (t.is_cuda and t.dtype == torch.float32 and t.dim() == 2):
+        raise TypeError(f"{name}: expected a CUDA float32 [N, D] tensor (any strides)")
+    return t.stride(0), t.stride(1)
+
+
+def amp_state_init(motion_lib, reset_mask, root_states, dof_pos, dof_vel, progress, reset_buf, terminate_buf, kind_out, motion_id_out,
+                   motion_time_out, state_init='Hybrid', hybrid_prob=0.5, recovery_prob=0.0, fall_prob=0.0, recovery_steps=0,
+                   init_root_states=None, init_dof_pos=None, init_dof_vel=None, fall_root_states=None, fall_dof_pos=None, fall_dof_vel=None,
+                   recovery_counter=None, rng=None, stream_id=0, recovery_in=None, fall_in=None, hybrid_in=None, motion_id_in=None,
+                   phase_in=None, fall_row_in=None):
+    """HumanoidAMP / HumanoidAMPGetup._reset_actors for the envs flagged in the uint8 reset_mask, without index lists.  root_states [N, 13] rows
+    and dof_pos / dof_vel [N, D] may be strided views (Isaac Gym's _root_states with two actors, the interleaved [N, D, 2] _dof_state); they
+    are written in place.  Draws come from the Philox stream {rng, stream_id} or from the injected per-env outcomes."""
+    n = reset_mask.shape[0]
+    rs = _rows(root_states, 'root_states')
+    dps, dpe = _dof_strides(dof_pos, 'dof_pos'); dvs, dve = _dof_strides(dof_vel, 'dof_vel')
+    assert progress.dtype == torch.int64 and reset_buf.dtype == torch.uint8 and terminate_buf.dtype == torch.uint8
+    assert kind_out.dtype == torch.uint8 and motion_id_out.dtype == torch.int32 and motion_time_out.dtype == torch.float32
+    assert recovery_counter is None or recovery_counter.dtype == torch.int32
+    for t in (init_root_states, init_dof_pos, init_dof_vel, fall_root_states, fall_dof_pos, fall_dof_vel):
+        assert t is None or (t.is_contiguous() and t.dtype == torch.float32)
+    p = L.StateInitParams(L.STATE_INIT[state_init], float(hybrid_prob), float(recovery_prob), float(fall_prob), int(recovery_steps),
+                          _p(reset_mask), n, _p(root_states), rs, _p(dof_pos), dps, dpe, _p(dof_vel), dvs, dve,
+                          _p(init_root_states), _p(init_dof_pos), _p(init_dof_vel), _p(fall_root_states), _p(fall_dof_pos), _p(fall_dof_vel),
+                          0 if fall_root_states is None else fall_root_states.shape[0], _p(recovery_counter), _p(progress), _p(reset_buf),
+                          _p(terminate_buf), _p(kind_out), _p(motion_id_out), _p(motion_time_out), _p(rng), int(stream_id),
+                          _p(recovery_in), _p(fall_in), _p(hybrid_in), _p(motion_id_in), _p(phase_in), _p(fall_row_in))
+    mp = motion_lib._params()
+    check(lib.ase_amp_state_init(C.byref(mp), _p(motion_lib._motion_cdf), motion_lib.num_motions(), C.byref(p), _stream()), 'ase_amp_state_init')
+
+
+def amp_history_init(motion_lib, kind, motion_ids, motion_times, amp_obs_buf, sim_dt, local_root_obs=True, root_height_obs=True):
+    """HumanoidAMP._init_amp_obs (+ the getup override) after slot 0 of the reset envs was rebuilt: default / fall envs repeat slot 0,
+    reference-init envs get their clip's frames at time - k dt; amp_obs_buf [N, S, step_dim] contiguous."""
+    assert amp_obs_buf.is_contiguous() and amp_obs_buf.dim() == 3
+    n, s, _ = amp_obs_buf.shape
+    mp = motion_lib._params()
+    check(lib.ase_amp_history_init(C.byref(mp), _p(kind), _p(motion_ids), _p(motion_times), n, float(sim_dt), int(bool(local_root_obs)),
+                                   int(bool(root_height_obs)), _p(amp_obs_buf), s, _stream()), 'ase_amp_history_init')
+
+
+def recovery_step(recovery_counter, reset_buf, terminate_buf):
+    """HumanoidAMPGetup._update_recovery_count + its _compute_reset override, after the env's reset rule."""
+    assert recovery_counter.dtype == torch.int32 and reset_buf.dtype == torch.uint8 and terminate_buf.dtype == torch.uint8
+    check(lib.ase_recovery_step(_p(recovery_counter), _p(reset_buf), _p(terminate_buf), recovery_counter.shape[0], _stream()), 'ase_recovery_step')

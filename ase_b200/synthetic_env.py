@@ -11,7 +11,12 @@ history, resets -- runs through the CUDA kernels exactly as post_physics_step wo
 `task` (HumanoidHeading / HumanoidLocation / HumanoidReach / HumanoidStrike, env/tasks/humanoid_<task>.py): the task observation is
 appended behind the humanoid features, the task reward replaces the zero reward, and targets are resampled on the device the way
 _update_task / _reset_task / _reset_target do, with in-kernel Philox draws (no host sync, CUDA-graph capturable).  `heading_task=True` is
-the older heading stand-in with FIXED targets (no resampling) and stays as it was."""
+the older heading stand-in with FIXED targets (no resampling) and stays as it was.
+
+`state_init` ('Default' / 'Start' / 'Random' / 'Hybrid', HumanoidAMP.StateInit) and `getup` (HumanoidAMPGetup) start episodes the way the
+reference's pre-training tasks do, on the device with in-kernel Philox draws: reset envs get the initial state, a reference state of a
+motion clip (their AMP history then holds the clip's previous frames) or, with `getup`, a lying-down state of a fall-state bank or a
+recovery episode that keeps its state; `dones` are suppressed while a recovery counter runs.  None (the default) keeps the plain reset."""
 import numpy as np
 import torch
 
@@ -39,7 +44,13 @@ class SyntheticHumanoidEnv:
 
     def __init__(self, num_envs, device='cuda', seed=0, pool=8, state_source='device', done_prob=1.0 / 300.0,
                  local_root_obs=True, root_height_obs=True, demo_pool=8192, heading_task=False, dt=1.0 / 30.0, demo_source='motion_lib',
-                 task=None):
+                 task=None, state_init=None, getup=False):
+        if state_init is not None and state_init not in ('Default', 'Start', 'Random', 'Hybrid'):
+            raise ValueError(f"state_init must be None, 'Default', 'Start', 'Random' or 'Hybrid', got {state_init!r}")
+        if state_init is not None and demo_source != 'motion_lib':
+            raise ValueError("state_init needs demo_source='motion_lib' (reference-state init samples the motion library)")
+        if getup and state_init is None:
+            raise ValueError("getup=True needs a state_init")
         if task is not None and heading_task:
             raise ValueError("heading_task=True (fixed targets) and task=... (resampled targets) exclude each other")
         if task is not None and task not in ops.TASK_OBS_SIZE:
@@ -111,6 +122,9 @@ class SyntheticHumanoidEnv:
         if task is not None:
             self._init_task(seed)
         self._load_state()
+        self.state_init, self.getup = state_init, getup
+        if state_init is not None:
+            self._init_resets(seed)
         if heading_task or task is not None:
             self._prev_root_pos.copy_(self._body[:, 0, 0:3])
         if task is not None:      # every env starts with a sampled target (HumanoidAMPTask._reset_envs -> _reset_task at the first reset)
@@ -185,6 +199,10 @@ class SyntheticHumanoidEnv:
         r = torch.rand(self.num_envs, device=self.device) if self.device.type == 'cuda' else torch.rand(self.num_envs, generator=self._gen)
         torch.lt(r, self.done_prob, out=self._done_bool); torch.lt(r, 0.5 * self.done_prob, out=self._term_bool)
         self.reset_buf.copy_(self._done_bool); self._terminate_buf.copy_(self._term_bool)        # terminate is a subset of dones
+        if self.getup:
+            ops.recovery_step(self._recovery_counter, self.reset_buf, self._terminate_buf)       # no reset while a recovery counter runs
+        if self.state_init is not None:
+            self._reset_rng[1:].add_(1)                     # every reset draw of this step has been taken (a launch of its own)
         self.extras['terminate'] = self._terminate_buf
         self.extras['amp_obs'] = self._amp_obs_buf.view(self.num_envs, -1)
         return self.obs_buf, self.rew_buf, self.reset_buf, self.extras
@@ -195,6 +213,11 @@ class SyntheticHumanoidEnv:
         (humanoid.py:125-128), an empty list none."""
         if env_ids is None:
             env_ids = torch.arange(self.num_envs, device=self.device)
+        if self.state_init is not None:
+            if len(env_ids) > 0:
+                mask = torch.zeros(self.num_envs, dtype=torch.uint8, device=self.device); mask[env_ids] = 1
+                self.reset_done(mask)
+            return self.obs_buf
         if len(env_ids) > 0:
             ids = env_ids.to(torch.int32)
             self.task.progress_buf[env_ids] = 0
@@ -211,13 +234,61 @@ class SyntheticHumanoidEnv:
 
     def reset_done(self, mask):
         """The same reset driven by a uint8 [N] mask on the device: no index list, no host sync (the agents use it when the env offers it)."""
-        self.task.progress_buf.masked_fill_(mask.bool(), 0)
+        if self.state_init is None:
+            self.task.progress_buf.masked_fill_(mask.bool(), 0)
+        else:
+            self._init_state(mask)                # _reset_actors + the zeroing of _reset_env_tensors
         if self.task_name == 'strike':            # _reset_target runs inside _reset_actors, before the observation is built
             self._resample_task(mask)
-        self._compute_observations(shift=False, env_mask=mask, fill_history=True)
+        self._compute_observations(shift=False, env_mask=mask, fill_history=self.state_init is None)
+        if self.state_init is not None:           # _init_amp_obs: history of the reset envs from their init kind
+            ops.amp_history_init(self._motion_lib, self._reset_kind, self._reset_motion_id, self._reset_motion_time, self._amp_obs_buf, self.dt,
+                                 self.local_root_obs, self.root_height_obs)
         if self.task_name is not None and self.task_name != 'strike':
             self._resample_task(mask)             # HumanoidAMPTask._reset_envs: _reset_task after the observation (it carries the old target)
         return self.obs_buf
+
+    # ---- episode starts of HumanoidAMP / HumanoidAMPGetup (state_init=..., getup=...) ------------------------------------------------
+    def _init_resets(self, seed, num_fall_states=64):
+        """The initial state (Default init), a fall-state bank and the reset buffers.  The reference simulates 150 steps of random actions to
+        collect fallen states (_generate_fall_states); here the bank is synthetic: lying-down roots (a random heading, rolled or pitched by
+        about 90 degrees, 0.1 - 0.3 m high) with random joint angles and zero velocities."""
+        n, D, dev = self.num_envs, self.NUM_DOFS, self.device
+        self._init_root = self._body[:, 0].clone()
+        self._init_dof_pos, self._init_dof_vel = self._dof[:, :D].clone(), self._dof[:, D:].clone()
+        g = torch.Generator().manual_seed(seed + 7717)
+        F = num_fall_states
+        yaw = torch.rand(F, generator=g) * 6.2831853
+        tilt = (1.5707963 + 0.2 * torch.randn(F, generator=g)) * torch.where(torch.rand(F, generator=g) < 0.5, -1.0, 1.0)
+        axis = torch.where((torch.rand(F, generator=g) < 0.5).unsqueeze(-1), torch.tensor([1.0, 0.0, 0.0]), torch.tensor([0.0, 1.0, 0.0]))
+        q_tilt = torch.cat([axis * torch.sin(tilt / 2).unsqueeze(-1), torch.cos(tilt / 2).unsqueeze(-1)], dim=-1)
+        q_yaw = torch.stack([torch.zeros(F), torch.zeros(F), torch.sin(yaw / 2), torch.cos(yaw / 2)], dim=-1)
+        x1, y1, z1, w1 = q_yaw.unbind(-1); x2, y2, z2, w2 = q_tilt.unbind(-1)
+        rot = torch.stack([w1 * x2 + x1 * w2 + y1 * z2 - z1 * y2, w1 * y2 + y1 * w2 + z1 * x2 - x1 * z2,
+                           w1 * z2 + z1 * w2 + x1 * y2 - y1 * x2, w1 * w2 - x1 * x2 - y1 * y2 - z1 * z2], dim=-1)
+        root = torch.zeros(F, 13)
+        root[:, 0:2] = torch.randn(F, 2, generator=g)
+        root[:, 2] = 0.1 + 0.2 * torch.rand(F, generator=g)
+        root[:, 3:7] = torch.nn.functional.normalize(rot, dim=-1)
+        self._fall_root = root.to(dev)
+        self._fall_dof_pos = (0.6 * (torch.rand(F, D, generator=g) * 2 - 1)).to(dev)
+        self._fall_dof_vel = torch.zeros(F, D, device=dev)
+        self._recovery_counter = torch.zeros(n, dtype=torch.int32, device=dev)
+        self._reset_kind = torch.zeros(n, dtype=torch.uint8, device=dev)
+        self._reset_motion_id = torch.zeros(n, dtype=torch.int32, device=dev)
+        self._reset_motion_time = torch.zeros(n, dtype=torch.float32, device=dev)
+        self._reset_rng = torch.tensor([seed * 6151 + 2017, 0], dtype=torch.int64, device=dev)       # {seed, step counter} of the Philox stream
+        self._state_init_params = dict(ops.STATE_INIT_PARAMS['getup' if self.getup else 'amp'], state_init=self.state_init)
+
+    def _init_state(self, mask):
+        """ase_amp_state_init on the env's own root (body 0 of the rigid-body state) and dof halves."""
+        D = self.NUM_DOFS
+        ops.amp_state_init(self._motion_lib, mask, self._body[:, 0], self._dof[:, :D], self._dof[:, D:], self.task.progress_buf, self.reset_buf,
+                           self._terminate_buf, self._reset_kind, self._reset_motion_id, self._reset_motion_time,
+                           init_root_states=self._init_root, init_dof_pos=self._init_dof_pos, init_dof_vel=self._init_dof_vel,
+                           fall_root_states=self._fall_root, fall_dof_pos=self._fall_dof_pos, fall_dof_vel=self._fall_dof_vel,
+                           recovery_counter=self._recovery_counter if self.getup else None, rng=self._reset_rng, stream_id=0,
+                           **self._state_init_params)
 
     # ---- the location / reach / strike tasks and device-side resampling for all four (task=...) ------------------------------------
     def _init_task(self, seed):

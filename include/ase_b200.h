@@ -181,7 +181,9 @@ int ase_policy_sample(const float* mu, const float* logstd, const float* noise, 
  * (a cos, a sin, b cos, b sin) with radii from x and z, angles from y and w) take u as it is.  The Bernoulli draw (stream sid + 1, group
  * 0xFFFFFFFF, word x: u < p) and the task uniforms (stream sid, group 0, words x..w) take min(u, 1 - 2^-24), in (0, 1) like torch.rand,
  * so p = 1 always gives 1 and a target never reaches the top of its range.  Randints (stream sid + 1, group 0xFFFFFFFE, word x) are
- * min + x % max(1, max - min).  oracle/philox_oracle.py restates all of it. */
+ * min + x % max(1, max - min).  The episode resets (ase_amp_state_init) follow the same rules: their uniforms (stream sid, groups 0 and 1)
+ * take min(u, 1 - 2^-24) and their fall-bank row is a randint (stream sid + 1, group 0xFFFFFFFE, word x).  oracle/philox_oracle.py restates
+ * all of it (oracle/getup_oracle.py the reset draws). */
 /* get_action_values' sampling half (rl_games ModelA2CContinuousLogStd eval + amp_agent.py:164-167): a = mu + exp(logstd) * noise,
  * rand_action_mask = bernoulli(rand_probs) (all ones when rand_probs is NULL), masked rows act deterministically. */
 int ase_policy_sample_rng(const float* mu, const float* logstd, const float* rand_probs, int rows, int act_dim,
@@ -234,6 +236,65 @@ typedef struct {
 int ase_task_resample(const AseTaskParams* p, const float* root_states, int64_t root_stride, const int64_t* progress, const uint8_t* reset_mask,
                       int num_envs, float* tar, int64_t tar_stride, float* tar_speed, float* tar_face_dir, int64_t* change_steps,
                       const uint64_t* rng, int stream_id, const float* u_in, const int64_t* steps_in, void* stream);
+
+/* ---- episode resets of HumanoidAMP / HumanoidAMPGetup without host syncs -------------------------------------------------------------
+ * The reference starts an episode with index lists (bernoulli -> env_ids[mask] -> len(...) > 0, multinomial for the clip ids): a host sync
+ * per sim step.  Three mask-driven entry points replace it, in this order for a reset:
+ *   ase_amp_state_init    HumanoidAMP._reset_actors / _reset_default / _reset_ref_state_init / _reset_hybrid_state_init / _set_env_state
+ *                         (env/tasks/humanoid_amp.py:141-201,238-246), HumanoidAMPGetup._reset_actors / _reset_recovery_episode /
+ *                         _reset_fall_episode (env/tasks/humanoid_amp_getup.py:78-116) and the buffer zeroing of
+ *                         Humanoid._reset_env_tensors (env/tasks/humanoid.py:150-167);
+ *   then ase_obs_build and ase_amp_obs_build (env_mask = reset_mask, no shift, no fill) rebuild the observation and AMP slot 0;
+ *   ase_amp_history_init  HumanoidAMP._init_amp_obs / _init_amp_obs_default / _init_amp_obs_ref (humanoid_amp.py:203-236) and the getup
+ *                         override (humanoid_amp_getup.py:123-129).
+ * Every step, after the env's reset rule (ase_humanoid_reset):
+ *   ase_recovery_step     HumanoidAMPGetup._update_recovery_count (pre_physics_step, humanoid_amp_getup.py:36-40,131-134) and its
+ *                         _compute_reset override (:136-142).  The decrement runs at post-physics here; that is equivalent because nothing
+ *                         reads the counter between pre_physics_step and _compute_reset.
+ * Init kinds, decided per env flagged in reset_mask in the reference's order: recovery (bernoulli(recovery_prob) and terminate[env]: the state
+ * is left as it is, counter := recovery_steps), else fall (bernoulli(fall_prob): root state, dof pos and dof vel := row randint(0, F) of the
+ * fall-state bank, counter := recovery_steps), else by state_init: Default (the env's initial root state and dofs), Start (reference state at
+ * time 0), Random (reference state at phase * motion_length), Hybrid (bernoulli(hybrid_prob): Random-style reference init, else Default);
+ * counter := 0 in these cases.  The reference clip id is the first m with u < motion_cdf[m] (inverse CDF; motion_cdf [M] is the fp32 cumsum
+ * of the normalised clip weights with the last entry 1.0, the role of torch.multinomial).  progress, reset and terminate := 0 for every
+ * flagged env.  Unflagged envs, and the state of recovery envs, are not written.
+ * Philox draws of env e (rng / stream_id as ase_latent_update; the caller advances rng[1] in a later launch): stream sid, group 0, words x, y,
+ * z, w = the recovery, fall and hybrid Bernoulli uniforms and the phase; stream sid, group 1, word x = the clip-id uniform; all through
+ * min(u, 1 - 2^-24) (so p = 1 always fires).  Fall row: stream sid + 1, group 0xFFFFFFFE, word x: x % max(1, F).
+ * Injected draws (per env, the outcomes torch.bernoulli / torch.multinomial / torch.rand / torch.randint_like record in the reference):
+ * recovery_in, fall_in, hybrid_in [N] uint8, motion_id_in [N] int32, phase_in [N] fp32, fall_row_in [N] int32. */
+typedef enum { ASE_STATE_INIT_DEFAULT = 0, ASE_STATE_INIT_START = 1, ASE_STATE_INIT_RANDOM = 2, ASE_STATE_INIT_HYBRID = 3 } AseStateInit;
+typedef enum { ASE_INIT_NONE = 0, ASE_INIT_DEFAULT = 1, ASE_INIT_REF = 2, ASE_INIT_FALL = 3, ASE_INIT_RECOVERY = 4 } AseInitKind;
+typedef struct {
+  int state_init;                          /* AseStateInit (stateInit) */
+  float hybrid_prob;                       /* hybridInitProb */
+  float recovery_prob, fall_prob;          /* recoveryEpisodeProb, fallInitProb (0 for plain HumanoidAMP) */
+  int recovery_steps;                      /* recoverySteps */
+  const uint8_t* reset_mask; int num_envs;
+  /* env state, written in place: root rows [N, 13] (pos, quat xyzw, vel, ang vel) root_stride floats apart (26 for Isaac Gym's two-actor
+   * _root_states); dof pos / vel [N, D] with row and element strides (Isaac Gym's [N, D, 2] _dof_state: row 2D, element 2) */
+  float* root_states; int64_t root_stride;
+  float* dof_pos; int64_t dof_pos_stride, dof_pos_elem_stride;
+  float* dof_vel; int64_t dof_vel_stride, dof_vel_elem_stride;
+  const float* init_root_states; const float* init_dof_pos; const float* init_dof_vel;    /* [N, 13], [N, D], [N, D] contiguous */
+  const float* fall_root_states; const float* fall_dof_pos; const float* fall_dof_vel;    /* [F, 13], [F, D], [F, D] contiguous */
+  int num_fall_states;                     /* F (0: no fall bank; fall_prob must then be 0) */
+  int32_t* recovery_counter;               /* [N] or NULL (plain HumanoidAMP) */
+  int64_t* progress; uint8_t* reset_buf; uint8_t* terminate_buf;                          /* [N]; terminate is read before it is cleared */
+  uint8_t* kind_out; int32_t* motion_id_out; float* motion_time_out;                      /* [N]: AseInitKind of every env (NONE when not
+                                                                                              flagged); clip id and time of REF envs */
+  const uint64_t* rng; int stream_id;
+  const uint8_t* recovery_in; const uint8_t* fall_in; const uint8_t* hybrid_in;
+  const int32_t* motion_id_in; const float* phase_in; const int32_t* fall_row_in;
+} AseStateInitParams;
+int ase_amp_state_init(const AseMotionLib* m, const float* motion_cdf, int num_motions, const AseStateInitParams* p, void* stream);
+/* After slot 0 of the flagged envs was rebuilt: DEFAULT and FALL envs get slots 1..S-1 := slot 0; REF envs get slot k := the AMP observation of
+ * their clip at time + fp32(-sim_dt * k), k = 1..S-1 (bitwise what ase_amp_obs_demo gives for that time with one step; times before the clip
+ * start extrapolate with a negative blend, as the reference does); NONE and RECOVERY envs are untouched.  amp_obs [N, S, step_dim]. */
+int ase_amp_history_init(const AseMotionLib* m, const uint8_t* kind, const int32_t* motion_ids, const float* motion_times, int num_envs,
+                         float sim_dt, int local_root_obs, int root_height_obs, float* amp_obs, int hist_steps, void* stream);
+/* counter := max(counter - 1, 0); then reset := 0 and terminate := 0 wherever counter > 0. */
+int ase_recovery_step(int32_t* recovery_counter, uint8_t* reset_buf, uint8_t* terminate_buf, int num_envs, void* stream);
 
 /* _calc_advs amp_agent.py:551-561 (+ torch_ext.normalization_with_masks); mask NULL => plain
  * mean / unbiased std (common_agent.py:536-546).  scratch >= 64 bytes. */
