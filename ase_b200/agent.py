@@ -691,7 +691,7 @@ class CommonAgent:
                                        "two consecutive calls; rerun with gemm_backend=1 (restore() the last checkpoint)")
                 rs, ls, cnt = (r['scalars'].pop(k, 0.0) for k in ('ep_reward_sum', 'ep_length_sum', 'ep_count'))
                 if cnt > 0:       # common_agent.py:125-136 (mean over the episodes that finished in this epoch)
-                    r['mean_rewards'], r['mean_lengths'] = rs / cnt, ls / cnt
+                    r['mean_rewards'], r['mean_lengths'] = self._get_mean_rewards(rs, cnt), ls / cnt
                     self.mean_rewards = r['mean_rewards']
                 total_time += r.get('play_time', 0.0) + r.get('update_time', 0.0)
                 r['total_time'] = total_time
@@ -723,6 +723,10 @@ class CommonAgent:
                     self.save(model_output_file)
                 self.total_time = total_time
                 return self.last_mean_rewards, epoch_num
+
+    def _get_mean_rewards(self, reward_sum, count):
+        """common_agent.py:466-467: the mean accumulated reward of the finished episodes."""
+        return reward_sum / count
 
     def _write_stats(self, r):
         """TensorBoard emission (common_agent.py:119-152, amp_agent.py:244-262) from an AsyncEpochLog record."""
@@ -1025,6 +1029,11 @@ class HRLAgent(CommonAgent):
         infos['terminate'] = (terminate_count > 0).to(torch.uint8)
         infos['disc_rewards'] = disc_rewards
         return {'obs': obs}, rewards.unsqueeze(1), (done_count > 0).to(torch.uint8), infos
+
+    def _get_mean_rewards(self, reward_sum, count):
+        """hrl_agent.py:172-175: an episode accumulates the per-step MEAN of the llc_steps sub-step rewards; the logged value is scaled back
+        to a sum over sub-steps."""
+        return super()._get_mean_rewards(reward_sum, count) * self._llc_steps
 
     def _extra_buffer_writes(self, n, res, infos):
         self.experience_buffer['disc_rewards'][n] = infos['disc_rewards']

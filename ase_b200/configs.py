@@ -48,8 +48,9 @@ AMP_HUMANOID = {   # amp_humanoid.yaml
 HRL_HUMANOID = {   # hrl_humanoid.yaml (HumanoidHeading / Location / Reach / Strike task training over a frozen LLC)
     'net_params': {
         'separate': True,
+        # the HLC explores wider than the LLC: log-std -2.3 (hrl_humanoid.yaml; the shipped HLC checkpoints store a2c_network.sigma = -2.3)
         'space': {'continuous': {'mu_activation': 'None', 'sigma_activation': 'None', 'mu_init': {'name': 'default'},
-                                 'sigma_init': {'name': 'const_initializer', 'val': -2.9}, 'fixed_sigma': True, 'learn_sigma': False}},
+                                 'sigma_init': {'name': 'const_initializer', 'val': -2.3}, 'fixed_sigma': True, 'learn_sigma': False}},
         'mlp': {'units': [1024, 512], 'activation': 'relu'},
     },
     'llc_net_params': ASE_HUMANOID['net_params'], 'latent_dim': 64,

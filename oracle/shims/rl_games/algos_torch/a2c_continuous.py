@@ -1,4 +1,5 @@
 """[recollection of rl_games 1.1.4 algos_torch/a2c_continuous.py] -- only what CommonAgent inherits."""
+from rl_games.algos_torch import torch_ext
 from rl_games.common import a2c_common
 
 
@@ -15,7 +16,8 @@ class A2CAgent(a2c_common.ContinuousA2CBase):
         return self.train_result
 
     def restore(self, fn):
-        raise NotImplementedError
+        checkpoint = torch_ext.load_checkpoint(fn)
+        self.set_full_state_weights(checkpoint)
 
     def save(self, fn):
         pass

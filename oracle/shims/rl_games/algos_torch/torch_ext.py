@@ -10,6 +10,12 @@ numpy_to_torch_dtype_dict = {
 }
 
 
+def load_checkpoint(filename):
+    print("=> loading checkpoint '{}'".format(filename))
+    state = torch.load(filename, map_location='cpu', weights_only=False)
+    return state
+
+
 def policy_kl(p0_mu, p0_sigma, p1_mu, p1_sigma, reduce=True):
     c1 = torch.log(p1_sigma / p0_sigma + 1e-5)
     c2 = (p0_sigma ** 2 + (p1_mu - p0_mu) ** 2) / (2.0 * (p1_sigma ** 2 + 1e-5))

@@ -53,7 +53,8 @@ class A2CBase:
         if self.env_info is None:
             self.vec_env = vecenv.create_vec_env(self.env_name, self.num_actors, **self.env_config)
             self.env_info = self.vec_env.get_env_info()
-        self.ppo_device = config.get('device', 'cuda:0')
+        # rl_games defaults to cuda:0; this CPU harness falls back to the CPU for configs that name no device (HRLAgent's LLC config)
+        self.ppo_device = config.get('device', 'cuda:0' if torch.cuda.is_available() else 'cpu')
         self.value_size = self.env_info.get('value_size', 1)
         self.observation_space = self.env_info['observation_space']
         self.weight_decay = config.get('weight_decay', 0.0)
@@ -163,6 +164,17 @@ class A2CBase:
 
     def preprocess_actions(self, actions):
         return actions
+
+    def get_action_values(self, obs):
+        """(HRLAgent.play_steps samples its actions here; AMPAgent / ASEAgent override it.)"""
+        processed_obs = self._preproc_obs(obs['obs'])
+        self.model.eval()
+        input_dict = {'is_train': False, 'prev_actions': None, 'obs': processed_obs, 'rnn_states': self.rnn_states}
+        with torch.no_grad():
+            res_dict = self.model(input_dict)
+        if self.normalize_value:
+            res_dict['values'] = self.value_mean_std(res_dict['values'], True)
+        return res_dict
 
     def env_step(self, actions):
         actions = self.preprocess_actions(actions)

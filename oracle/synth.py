@@ -82,6 +82,77 @@ def rollout_script(fx=None, g=None, N=16, H=8):
     return dict(obs_t=obs_t, reset_obs_t=reset_obs_t, amp_t=amp_t) if fx is not None else (rms, obs_t, reset_obs_t, amp_t)
 
 
+HRL_LLC_PARAM_SEED, HRL_HLC_PARAM_SEED = 31, 13
+
+
+def hrl_llc_params():
+    """Seeded weights of the LLC behind tests/golden/rollout_hrl.pt: the ASE network at production widths."""
+    return params(O.ase_param_shapes(), seed=HRL_LLC_PARAM_SEED)
+
+
+def hrl_hlc_params():
+    """Seeded weights of the HLC behind tests/golden/rollout_hrl.pt (hrl_humanoid.yaml: obs 258, act 64, units [1024, 512]).  No sigma:
+    the network's log-std is the config's constant."""
+    p = params(O.amp_param_shapes(obs=258, act=64, amp=0, units=(1024, 512)), seed=HRL_HLC_PARAM_SEED)
+    del p['sigma']
+    return p
+
+
+def hrl_rollout_script(fx=None, N=24, H=6, llc_steps=5):
+    """Normaliser statistics and per-LLC-step env tables of the scripted env behind tests/golden/rollout_hrl.pt (K = llc_steps * H sub-steps).
+    The LLC statistics are the shipped checkpoint's (tests/golden/inference_shipped_stats.pt); the HLC observation statistics extend them by
+    the 5 task dims.  Observations lie around the LLC mean with 1.5 x its standard deviations, some rows 40 standard deviations off; AMP
+    observations likewise, plus rows pushed 40 standard deviations along the sign of the discriminator's input gradient, whose logits sit
+    far beyond the 1e-4 floor of `1 - prob`.  Dones and terminations hit the first, a middle and the last sub-step of an HLC step and the
+    rollout's last sub-step."""
+    import os
+    if fx is not None:
+        N, H, llc_steps = fx['N'], fx['H'], fx['llc_steps']
+    K = H * llc_steps
+    golden = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'tests', 'golden')
+    shipped = torch.load(os.path.join(golden, 'inference_shipped_stats.pt'), weights_only=False)['rms']
+    llc_rms = {k: {kk: vv.clone() for kk, vv in v.items()} for k, v in shipped.items()}
+    g = torch.Generator().manual_seed(91)
+    m, sd = llc_rms['running_mean_std']['running_mean'].float(), llc_rms['running_mean_std']['running_var'].float().sqrt()
+    ma, sda = llc_rms['amp_input_mean_std']['running_mean'].float(), llc_rms['amp_input_mean_std']['running_var'].float().sqrt()
+
+    def obs_rows(*shape):
+        return torch.cat([m + 1.5 * sd * torch.randn(*shape, 253, generator=g), torch.randn(*shape, 5, generator=g) * 2.0], dim=-1)
+    hlc_rms = {'running_mean_std': {'running_mean': torch.cat([llc_rms['running_mean_std']['running_mean'], 0.3 * torch.randn(5, generator=g).double()]),
+                                    'running_var': torch.cat([llc_rms['running_mean_std']['running_var'], (0.5 + torch.rand(5, generator=g)).double() * 4.0]),
+                                    'count': torch.tensor(1000.0, dtype=torch.float64)},
+               'reward_mean_std': {'running_mean': 0.3 * torch.randn(1, generator=g).double(), 'running_var': (0.5 + torch.rand(1, generator=g)).double(),
+                                   'count': torch.tensor(1000.0, dtype=torch.float64)}}
+    obs_t = obs_rows(K + 1, N)
+    reset_obs_t = obs_rows(H + 1, N)
+    # LLC inputs (sub-steps 1..4 of an HLC step read the previous sub-step's observation) 40 standard deviations off the mean
+    obs_t[3, 5, :253] = m + 40.0 * sd
+    obs_t[7, 6, :253] = m - 40.0 * sd
+    obs_t[K - 1, 7, :253] = m + 40.0 * sd * torch.sign(torch.randn(253, generator=g))
+    amp_t = ma + 1.5 * sda * torch.randn(K, N, 1400, generator=g)
+    rew_t = torch.rand(K, N, generator=g)
+    dones_t = (torch.rand(K, N, generator=g) < 0.04).to(torch.uint8)
+    term_t = (dones_t.bool() & (torch.rand(K, N, generator=g) < 0.5)).to(torch.uint8)
+    # a done on the first (env 1), a middle (env 2) and the last (env 3) sub-step of an HLC step, a termination inside an HLC step (env 4),
+    # a done on the rollout's last sub-step (env 0)
+    dones_t[0 * llc_steps + 0, 1] = 1
+    dones_t[1 * llc_steps + 2, 2] = 1
+    dones_t[2 * llc_steps + llc_steps - 1, 3] = 1
+    dones_t[3 * llc_steps + 1, 4] = 1; term_t[3 * llc_steps + 1, 4] = 1
+    dones_t[K - 1, 0] = 1
+    # discriminator rows on the 1e-4 floor: normalised input at the +-5 clamp along the sign of d logit / d input at the mean
+    P = hrl_llc_params()
+    x = torch.zeros(1, 1400, dtype=torch.float64, requires_grad=True)
+    O.eval_disc({k: v.double() for k, v in P.items()}, x).sum().backward()
+    s = torch.sign(x.grad[0]).float()
+    amp_t[2, 9] = ma + 40.0 * sda * s
+    amp_t[K - 3, 10] = ma + 40.0 * sda * s
+    out = dict(obs_t=obs_t, reset_obs_t=reset_obs_t, amp_t=amp_t, rew_t=rew_t, dones_t=dones_t, term_t=term_t, llc_rms=llc_rms, hlc_rms=hlc_rms)
+    if fx is None:
+        out.update(N=N, H=H, llc_steps=llc_steps)
+    return out
+
+
 def shipped_stats_inputs(fx, n=96):
     """Inputs of tests/golden/inference_shipped_stats.pt: observations and AMP observations around the stored (shipped) normaliser
     statistics with 1.5 x their standard deviations, plus rows at the mean, 40 standard deviations away and just off the mean; unit
