@@ -8,9 +8,10 @@
 // wgmma descriptors -- nothing is transposed -- and are normally WRITTEN by the epilogue of the GEMM that produces the tensor.
 // wgmma reads 32-bit operands K-major only, so a TF32 operand stored [K, rows] is split into K-major planes by its prep pass.
 //
-// Kernel (gemm_tc_kernel, 128 x 128 or 128 x 64 output tile): warpgroup 0 = TMA producer into a shared-memory ring with
-// mbarrier completion; warpgroups 1, 2 = 64 rows each: wgmma into register fragments, every k-block's A_hi.B_hi partial added
-// into fp32 registers with round-to-nearest adds -- the tensor core's own accumulation truncates.
+// Kernel (gemm_tc_kernel, BM x BN output tile, BM = 256 or 128, BN = 128 or 64, chosen by gemm_tc_plan): warpgroup 0 = TMA
+// producer into a shared-memory ring with mbarrier completion; warpgroups 1, 2 = BM / 2 rows each: wgmma into register
+// fragments, every (k-block, m64 block)'s partial -- corrections and A_hi.B_hi -- added into fp32 registers with
+// round-to-nearest adds -- the tensor core's own accumulation truncates.
 // Store phase: registers -> shared staging tile -> coalesced pass with bias / ReLU / tanh / mask (fp32 or 1-bit), optional
 // fp32 C, half planes (predicted power-of-two scale), ReLU activity bits, max |C|, fused column sums, split-K fp32 RED.
 // Descriptor formats follow the PTX ISA "Matrix Descriptor Format" for wgmma.  DESIGN.md section 5 has the numerics.
@@ -129,13 +130,13 @@ __device__ __forceinline__ void epilogue_rows(const TcEpi& e, const float* cs, i
   }
 }
 
-// Fast store phase of the 128x256 kernel for interior, aligned tiles (the generic epilogue_rows above handles everything else).
+// Fast store phase for interior, aligned tiles of BN = 128 (the generic epilogue_rows above handles everything else).
 // The generic loop spends ~500 issue slots per (row, 4-column) item on predicates, 64-bit address arithmetic and scalar tails
 // (ncu r01b: 43 % of the kernel's lifetime, issue-bound, not memory-bound).  Here a lane owns 8 consecutive columns of each of the
 // warp's 16 rows: two LDS.128 from the staged tile, one 16-byte store per half plane, pointers advanced by the row strides, the
 // rows' activity-mask words prefetched before the loop, no bounds checks.
-__device__ __forceinline__ bool epilogue_fast_ok(const TcEpi& e, int m0, int n0, int bn, bool H) {
-  if (e.accumulate || m0 + TC_BM > e.M || n0 + bn > e.N) return false;
+__device__ __forceinline__ bool epilogue_fast_ok(const TcEpi& e, int m0, int n0, int bm, int bn, bool H) {
+  if (e.accumulate || m0 + bm > e.M || n0 + bn > e.N) return false;
   if ((e.ldc & 3) || (reinterpret_cast<uintptr_t>(e.C) & 15)) return false;
   if (e.bias && (reinterpret_cast<uintptr_t>(e.bias) & 15)) return false;
   if (e.Chi && (!H || (e.ldp & 7) || (reinterpret_cast<uintptr_t>(e.Chi) & 15) || (reinterpret_cast<uintptr_t>(e.Clo) & 15))) return false;
@@ -270,12 +271,16 @@ __device__ __forceinline__ void epilogue_fast(const TcEpi& e, const float* cs, i
   }
 }
 
-template <int BN, int STAGES>
+// Ring depth per tile shape: as many stages as fit in ~200 KB of the 227 KB an H100 block may use
+template <int BM, int BN> constexpr int tc_stages() { return (200 * 1024) / (256 * (BM + BN)); }
+
+template <int BM, int BN, int STAGES>
 struct TcSmem {
-  static constexpr int A_BYTES = TC_BM * 128;                // 16 KB per plane: one 128-byte k-block row per operand row
+  static constexpr int A_BYTES = BM * 128;                   // per plane: one 128-byte k-block row per operand row
   static constexpr int B_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
   static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(BM * (BN + 4) * 4 + BN * 4 <= STAGES * STAGE_BYTES, "the store phase's staging tile lives over the ring");
 };
 
 // one 64 x BN MMA over k-slice k (32 bytes of K) of a k-block; sd = 0 starts a fresh accumulator
@@ -291,29 +296,33 @@ __device__ __forceinline__ void wg_mma(float (&d)[BN / 2], uint32_t a, uint32_t 
 
 // fp32-exact accumulation ("accumulate outside the tensor core", Ootomo & Yokota 2022): the tensor core adds into its
 // accumulator with truncation, which over K/8 x 3 sequential MMAs costs ~1e-5 absolute on O(1) sums -- enough to flip ReLU
-// masks against the fp32 reference.  So the main term A_hi.B_hi is accumulated by the tensor core only WITHIN one k-block
-// (4 MMAs into a fresh register fragment); the partial is then added into a second fragment with round-to-nearest FADDs while
-// the tensor core works on the k-block's correction MMAs.  The two correction terms (2^-11 smaller) accumulate across all of K
-// in a third fragment: their truncation is negligible.
+// masks against the fp32 reference.  So the tensor core accumulates only WITHIN one k-block of 64 halfs / 32 TF32 words:
+// per m64 block the 8 correction MMAs (A_lo.B_hi, A_hi.B_lo; 2^-11 of the main term, the first one starting a fresh
+// fragment) come first, then the 4 main MMAs A_hi.B_hi add into the same partial, and the partial is added into the fp32
+// accumulator with round-to-nearest FADDs.  The main term sees 4 truncating adds per rounded add (one more than with a fresh
+// main partial) and the corrections no longer truncate across all of K.
 //
 // Warp specialisation: warpgroup 0 (register budget lowered to 40) is the TMA producer into a STAGES-deep shared-memory ring
-// with mbarrier completion; warpgroups 1 and 2 (232 registers: three 64 x BN fp32 fragments) each own 64 rows of the 128 x BN
-// tile, issue its wgmma, and run the store phase.
-template <int BN, int STAGES, bool AMN, bool BMN, bool H>
+// with mbarrier completion; warpgroups 1 and 2 (232 registers) each own BM / 2 rows of the BM x BN tile as BM / 128 m64
+// blocks -- at BM = 256 two 64 x BN accumulators plus one partial, 192 registers at BN = 128 -- issue their wgmma, and run
+// the store phase.  While one warpgroup waits for its partial and adds it, the other's MMAs keep the tensor core busy.
+template <int BM, int BN, int STAGES, bool AMN, bool BMN, bool H>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__ CUtensorMap tmAlo,
                const __grid_constant__ CUtensorMap tmBhi, const __grid_constant__ CUtensorMap tmBlo, const TcEpi e) {
   static_assert(H || (!AMN && !BMN), "TF32 wgmma reads K-major operands only");
-  using SM = TcSmem<BN, STAGES>;
+  static_assert(BM == 128 || BM == 256, "tile height");
+  using SM = TcSmem<BM, BN, STAGES>;
   using F = TcFmt<H>;
   constexpr int R = BN / 2;                        // fragment registers per thread (64 x BN fp32 over 128 threads)
+  constexpr int NH = BM / 128;                     // m64 blocks per consumer warpgroup
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * SM::STAGE_BYTES);
   uint64_t* empty = full + STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m0 = blockIdx.y * TC_BM, n0 = blockIdx.x * BN;
+  const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
   const int kb_begin = blockIdx.z * e.kb_per_split;
   const int nkb = min(e.kb_per_split, e.kb_total - kb_begin);
 
@@ -338,12 +347,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant_
         mbar_expect_tx(&full[s], SM::STAGE_BYTES);
         uint8_t* st = smem + s * SM::STAGE_BYTES;
         const int k0 = (kb_begin + kb) * F::BK;
-        if (!AMN) {          // K-major planes [rows, K]: one box of 128 rows x one k-block
+        if (!AMN) {          // K-major planes [rows, K]: one box of BM rows x one k-block
           tma_load_2d(st, &tmAhi, &full[s], k0, m0);
           tma_load_2d(st + SM::A_BYTES, &tmAlo, &full[s], k0, m0);
         } else {             // MN-major planes [K, rows]: boxes of BK k-rows x 128 bytes of m
 #pragma unroll
-          for (int b = 0; b < TC_BM / F::MN_BOX; ++b) {
+          for (int b = 0; b < BM / F::MN_BOX; ++b) {
             tma_load_2d(st + b * F::MN_BOX_BYTES, &tmAhi, &full[s], m0 + b * F::MN_BOX, k0);
             tma_load_2d(st + SM::A_BYTES + b * F::MN_BOX_BYTES, &tmAlo, &full[s], m0 + b * F::MN_BOX, k0);
           }
@@ -363,65 +372,70 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant_
     return;
   }
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-  const int wg = (warp >> 2) - 1;                  // consumer warpgroup: tile rows [64 wg, 64 wg + 64)
+  const int wg = (warp >> 2) - 1;                  // consumer warpgroup: tile rows [wg BM/2, (wg + 1) BM/2)
   const int t = threadIdx.x & 127;
-  float acc[R], part[R], corr[R];
+  const bool corrections = !(e.debug & 4);
+  float acc[NH][R], part[R];
 #pragma unroll
-  for (int j = 0; j < R; ++j) { acc[j] = 0.0f; corr[j] = 0.0f; }
+  for (int h = 0; h < NH; ++h)
+#pragma unroll
+    for (int j = 0; j < R; ++j) acc[h][j] = 0.0f;
   for (int kb = 0; kb < nkb; ++kb) {
     const int s = kb % STAGES;
     mbar_wait(&full[s], (kb / STAGES) & 1);
-    // this warpgroup's 64 A rows start 8 KB into each A plane in both layouts (64 K-major 128-byte rows / the second 64-wide MN box)
     const uint32_t sa = smem_u32(smem + s * SM::STAGE_BYTES);
-    const uint32_t a_hi = sa + wg * 8192, a_lo = a_hi + SM::A_BYTES, b_hi = sa + 2 * SM::A_BYTES, b_lo = b_hi + SM::B_BYTES;
-    wg_fence();
+    const uint32_t b_hi = sa + 2 * SM::A_BYTES, b_lo = b_hi + SM::B_BYTES;
 #pragma unroll
-    for (int k = 0; k < 4; ++k) wg_mma<BN, AMN, BMN, H>(part, a_hi, b_hi, k, k > 0 ? 1 : 0);
-    wg_commit();
-    if (!(e.debug & 4)) {
+    for (int h = 0; h < NH; ++h) {
+      // m64 block wg NH + h starts (wg NH + h) x 8 KB into each A plane in both layouts
+      const uint32_t a_hi = sa + (wg * NH + h) * TC_M64_BYTES, a_lo = a_hi + SM::A_BYTES;
+      wg_fence();
+      if (corrections) {
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        wg_mma<BN, AMN, BMN, H>(corr, a_lo, b_hi, k, 1);
-        wg_mma<BN, AMN, BMN, H>(corr, a_hi, b_lo, k, 1);
+        for (int k = 0; k < 4; ++k) {
+          wg_mma<BN, AMN, BMN, H>(part, a_lo, b_hi, k, k > 0 ? 1 : 0);
+          wg_mma<BN, AMN, BMN, H>(part, a_hi, b_lo, k, 1);
+        }
       }
-    }
-    wg_commit();
-    wg_wait<1>();                                  // this k-block's main partial and the previous k-block's corrections are done
-    if (kb > 0 && t == 0) mbar_arrive(&empty[(kb - 1) % STAGES]);
 #pragma unroll
-    for (int j = 0; j < R; ++j) acc[j] += part[j];     // round-to-nearest fp32 accumulation across k-blocks
+      for (int k = 0; k < 4; ++k) wg_mma<BN, AMN, BMN, H>(part, a_hi, b_hi, k, (corrections || k > 0) ? 1 : 0);
+      wg_commit();
+      wg_wait<0>();
+      if (h == NH - 1 && t == 0) mbar_arrive(&empty[s]);   // every MMA reading this stage is done
+#pragma unroll
+      for (int j = 0; j < R; ++j) acc[h][j] += part[j];    // round-to-nearest fp32 accumulation across k-blocks
+    }
   }
-  wg_wait<0>();
-  // Phase 1: (main + correction) -> shared staging tile [128][BN+4] over the idle ring (every TMA load was consumed; the
-  // barrier waits for the other warpgroup's last MMAs).  Fragment layout of m64nN: thread t holds rows 16 (t/32) + (t%32)/4
-  // (+8) and column pairs 8 j + 2 (t%4).
+  // Phase 1: accumulators -> shared staging tile [BM][BN+4] over the idle ring (every TMA load was consumed; the barrier
+  // waits for the other warpgroup's last MMAs).  Fragment layout of m64nN: thread t holds rows 16 (t/32) + (t%32)/4 (+8)
+  // and column pairs 8 j + 2 (t%4).
   asm volatile("bar.sync 1, 256;" ::: "memory");      // the 8 consumer warps only
   float* cs = reinterpret_cast<float*>(smem);
   constexpr int CS_LD = BN + 4;
   // FP16 planes: undo the operands' power-of-two scales (two exact multiplies; their product alone could underflow)
   const float s1 = (H && e.a_inv) ? *e.a_inv : 1.0f;
   const float s2 = e.alpha * ((H && e.b_inv) ? *e.b_inv : 1.0f);
-  {
-    const int row = wg * 64 + 16 * (t >> 5) + ((t & 31) >> 2);
+#pragma unroll
+  for (int h = 0; h < NH; ++h) {
+    const int row = (wg * NH + h) * 64 + 16 * (t >> 5) + ((t & 31) >> 2);
     float* c0 = cs + row * CS_LD + 2 * (t & 3);
 #pragma unroll
     for (int j = 0; j < R / 4; ++j) {
-      const float* a = acc + 4 * j; const float* c = corr + 4 * j;
-      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(smem_u32(c0 + 8 * j)),
-                   "f"(s2 * (s1 * (a[0] + c[0]))), "f"(s2 * (s1 * (a[1] + c[1]))) : "memory");
-      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(smem_u32(c0 + 8 * CS_LD + 8 * j)),
-                   "f"(s2 * (s1 * (a[2] + c[2]))), "f"(s2 * (s1 * (a[3] + c[3]))) : "memory");
+      const float* a = acc[h] + 4 * j;
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(smem_u32(c0 + 8 * j)), "f"(s2 * (s1 * a[0])), "f"(s2 * (s1 * a[1])) : "memory");
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(smem_u32(c0 + 8 * CS_LD + 8 * j)), "f"(s2 * (s1 * a[2])), "f"(s2 * (s1 * a[3])) : "memory");
     }
   }
-  float* s_colsum = cs + TC_BM * CS_LD;               // [BN] per-tile column sums, behind the staging tile
+  float* s_colsum = cs + BM * CS_LD;                  // [BN] per-tile column sums, behind the staging tile
   const int et = threadIdx.x - 128;                   // 0..255 within the consumer warps
   if (e.colsum && et < BN) s_colsum[et] = 0.0f;
   asm volatile("bar.sync 1, 256;" ::: "memory");
-  // Phase 2: coalesced epilogue -- consumer warp w owns rows [16w, 16w+16)
+  // Phase 2: coalesced epilogue -- consumer warp w owns rows [w BM/8, (w + 1) BM/8)
+  constexpr int NRW = BM / 8;
   const int ew = warp - 4;
   if (!(e.debug & 1)) {
-    if (BN == 128 && epilogue_fast_ok(e, m0, n0, BN, H) && !(e.debug & 256)) epilogue_fast<H, 4, 16>(e, cs, CS_LD, s_colsum, ew * 16, m0, n0, lane);
-    else epilogue_rows<H>(e, cs, CS_LD, s_colsum, ew * 16, 16, BN, m0, n0, lane);
+    if (BN == 128 && epilogue_fast_ok(e, m0, n0, BM, BN, H) && !(e.debug & 256)) epilogue_fast<H, 4, NRW>(e, cs, CS_LD, s_colsum, ew * NRW, m0, n0, lane);
+    else epilogue_rows<H>(e, cs, CS_LD, s_colsum, ew * NRW, NRW, BN, m0, n0, lane);
   }
   if (e.colsum && !e.accumulate) {
     asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -639,7 +653,7 @@ struct MapKeyHash {
 static std::unordered_map<MapKey, CUtensorMap, MapKeyHash>& map_cache() { static std::unordered_map<MapKey, CUtensorMap, MapKeyHash> c; return c; }
 
 // 2D map over [rows, cols] elements (cols contiguous, row stride ld elements); the box is one 128-byte row chunk
-// (32 fp32 words / 64 halfs) x box_rows
+// (32 fp32 words / 64 halfs) x box_rows, 128-byte swizzle
 static int encode_cached(CUtensorMap* tm, const void* base, int rows, int cols, int64_t ld, int box_rows, bool mn_major, bool half = false) {
   MapKey k{base, rows, cols, ld, box_rows, (mn_major ? 1 : 0) | (half ? 2 : 0)};
   auto& c = map_cache();
@@ -661,20 +675,28 @@ static int encode_cached(CUtensorMap* tm, const void* base, int rows, int cols, 
   return ASE_OK;
 }
 
-// 2D tensor map over a zero-padded plane [rows_p, cols_p] (cols contiguous); box = [box_rows x 32 cols], 128B swizzle
+// 2D tensor map over a zero-padded plane [rows_p, cols_p] (cols contiguous)
 static int make_map(CUtensorMap* tm, const void* base, int rows_p, int cols_p, int box_rows, bool mn_major = false, bool half = false) {
   return encode_cached(tm, base, rows_p, cols_p, cols_p, box_rows, mn_major, half);
 }
 
 static inline int pad_to(int x, int m) { return (x + m - 1) / m * m; }
 
-// planes are padded to whole tiles in both dimensions (zero filled by the prep kernel): no reliance on TMA OOB fill
+// planes are padded to whole tiles in both dimensions (zero filled by the prep kernel), M to the tallest tile (256 rows)
 // (the FP16 format needs half of it: [*, pad(K, 64)] halfs <= [*, pad(K, 32)] words; the first TC_WS_HEAD bytes hold the
 // amax / scale slots of a registry-less call)
+// amax / scale slots of a registry-less call).  The plane slots are sized in fp32 words of K padded to 32 in BOTH formats:
+// the split passes and gemm_tc place the planes with tc_ws_slots, the one layout gemm_tc_workspace_bytes sums up.
 constexpr int64_t TC_WS_HEAD = 1024;
+constexpr int TC_MPAD = 256;
+struct TcWsSlots { int64_t a, b; };      // bytes of one A plane slot / one B plane slot
+static TcWsSlots tc_ws_slots(int M, int N, int K) {
+  const int64_t Mp = pad_to(M, TC_MPAD), Np = pad_to(N, 128), Kw = pad_to(K, TC_KPAD);
+  return {align_up(Mp * Kw * 4, 1024), align_up(Np * Kw * 4, 1024)};
+}
 int64_t gemm_tc_workspace_bytes(int M, int N, int K) {
-  const int64_t Mp = pad_to(M, 128), Np = pad_to(N, 128), Kp = pad_to(K, TC_BK);
-  return TC_WS_HEAD + 2 * align_up(Mp * Kp * 4, 1024) + 2 * align_up(Np * Kp * 4, 1024);
+  const TcWsSlots s = tc_ws_slots(M, N, K);
+  return TC_WS_HEAD + 2 * s.a + 2 * s.b;
 }
 
 // every shape runs on the tensor cores (small heads are padded up to one tile)
@@ -757,16 +779,17 @@ int tc_pdl() {   // env ASE_TC_PDL=0 launches the GEMMs fully stream-serialised
   return v;
 }
 
-template <int BN, int STAGES, bool AMN, bool BMN, bool H>
+template <int BM, int BN, bool AMN, bool BMN, bool H>
 static int launch_tc(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl, const TcEpi& e,
                      int splits, cudaStream_t st) {
-  using SM = TcSmem<BN, STAGES>;
+  constexpr int STAGES = tc_stages<BM, BN>();
+  using SM = TcSmem<BM, BN, STAGES>;
   static bool attr_set = false;
   if (!attr_set) {
-    ASE_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BN, STAGES, AMN, BMN, H>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::TOTAL));
+    ASE_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BM, BN, STAGES, AMN, BMN, H>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::TOTAL));
     attr_set = true;
   }
-  dim3 grid(ceil_div(e.N, BN), ceil_div(e.M, TC_BM), splits);
+  dim3 grid(ceil_div(e.N, BN), ceil_div(e.M, BM), splits);
   const bool prof = g_prof.on;
   if (prof) prof_mark(st);
   cudaLaunchConfig_t cfg = {};
@@ -775,27 +798,60 @@ static int launch_tc(const CUtensorMap& ah, const CUtensorMap& al, const CUtenso
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = tc_pdl();
   cfg.attrs = attr; cfg.numAttrs = 1;
-  ASE_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, STAGES, AMN, BMN, H>, ah, al, bh, bl, e));
+  ASE_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BM, BN, STAGES, AMN, BMN, H>, ah, al, bh, bl, e));
   if (prof) { prof_mark(st); g_prof.flops += 2.0 * (double)e.M * (double)e.N * (double)e.K; }
   ASE_LAUNCH_OK();
   return ASE_OK;
 }
 
-template <int BN, int STAGES, bool H>
+template <int BM, int BN, bool H>
 static int launch_tc_major(bool amn, bool bmn, const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
                            const TcEpi& e, int splits, cudaStream_t st) {
   if constexpr (!H) {
     if (amn || bmn) { set_error("wgmma GEMM: TF32 operand planes must be K-major"); return ASE_ERR_INVALID; }
-    return launch_tc<BN, STAGES, false, false, false>(ah, al, bh, bl, e, splits, st);
+    return launch_tc<BM, BN, false, false, false>(ah, al, bh, bl, e, splits, st);
   } else {
-    if (!amn && !bmn) return launch_tc<BN, STAGES, false, false, true>(ah, al, bh, bl, e, splits, st);
-    if (!amn && bmn) return launch_tc<BN, STAGES, false, true, true>(ah, al, bh, bl, e, splits, st);
-    if (amn && !bmn) return launch_tc<BN, STAGES, true, false, true>(ah, al, bh, bl, e, splits, st);
-    return launch_tc<BN, STAGES, true, true, true>(ah, al, bh, bl, e, splits, st);
+    if (!amn && !bmn) return launch_tc<BM, BN, false, false, true>(ah, al, bh, bl, e, splits, st);
+    if (!amn && bmn) return launch_tc<BM, BN, false, true, true>(ah, al, bh, bl, e, splits, st);
+    if (amn && !bmn) return launch_tc<BM, BN, true, false, true>(ah, al, bh, bl, e, splits, st);
+    return launch_tc<BM, BN, true, true, true>(ah, al, bh, bl, e, splits, st);
   }
 }
 
-int gemm_tc_tile_n(int N) { return N > 64 ? 128 : 64; }
+static int tc_debug() {   // env ASE_TC_DEBUG: experiment bits, see TcEpi::debug
+  static int v = -1;
+  if (v < 0) { const char* d = getenv("ASE_TC_DEBUG"); v = d ? atoi(d) : 0; }
+  return v;
+}
+
+// Tile plan of one tensor-core GEMM: the tile height BM, the tile width BN and the number of K splits.  BN = 128, or 64
+// when N <= 64.  (BM, splits) minimise a launch-time model: whole waves of one-CTA-per-SM launches times the per-CTA time
+//   TC_CTA_FIXED + (k-blocks per split + TC_CTA_STORE) x BM BN / 128^2,
+// in units of one k-block of a 128 x 128 tile (12 MMAs per consumer warpgroup and m64 block): a CTA pays a fixed start (first TMA
+// round trip, barrier set-up) and a store phase that grows with its area.  Every extra split adds 3 % for its RED pass over C.
+// split_k > 1 (with accumulate) is taken as given, 0 / 1 is none; split_k < 0 (TC_SPLIT_AUTO, with accumulate: the learner's
+// dW GEMMs) lets the model pick up to 64 splits of at least 4 k-blocks each: the learner's small dW outputs (a few 128-row
+// tiles over K = 4096 .. 32768) need 16-64 splits to give every SM a CTA.  Without accumulate there is no split-K.
+constexpr double TC_CTA_FIXED = 1.0, TC_CTA_STORE = 1.0;
+TcPlan gemm_tc_plan(int M, int N, int K, int accumulate, int split_k, int sms, bool f16) {
+  TcPlan best{128, N > 64 ? 128 : 64, 1};
+  const int kb_total = ceil_div(K, f16 ? TcFmt<true>::BK : TcFmt<false>::BK);
+  int smin = 1, smax = 1;
+  if (accumulate && split_k > 1) smin = smax = min(split_k, kb_total);
+  else if (accumulate && split_k < 0) smax = max(1, min(64, kb_total / 4));
+  const int bm_max = (tc_debug() & 512) ? 128 : 256;
+  double best_cost = 1e300;
+  for (int bm = 128; bm <= bm_max; bm *= 2) {
+    for (int s = smin; s <= smax; ++s) {
+      const int kbs = ceil_div(kb_total, s), splits = ceil_div(kb_total, kbs);    // as launched: no empty split
+      const int64_t ctas = (int64_t)ceil_div(M, bm) * ceil_div(N, best.bn) * splits;
+      const double area = (double)bm * best.bn / (128.0 * 128.0);
+      const double cost = (double)ceil_div(ctas, (int64_t)sms) * (TC_CTA_FIXED + (kbs + TC_CTA_STORE) * area) * (1.0 + 0.03 * splits);
+      if (cost < best_cost - 1e-9) { best_cost = cost; best.bm = bm; best.splits = splits; }
+    }
+  }
+  return best;
+}
 
 // ---------------------------------------------------------------------------------------------------------
 // Operand-plane registry: fp32 buffers whose TF32 hi/lo planes are kept next to them so that a tensor is split at
@@ -944,10 +1000,12 @@ static int make_view_map(CUtensorMap* tm, const void* base, int rows, int cols, 
 int gemm_tc(const AseGemmParams& p, cudaStream_t st, PlaneRegistry* reg) {
   const bool H = p.backend == 2;             // scaled FP16 hi/lo planes instead of TF32 ones
   if (reg && reg->f16 != H) { set_error("wgmma GEMM: plane registry format does not match backend %d", p.backend); return ASE_ERR_INVALID; }
-  const int BK = H ? 64 : 32;
-  const int BN = gemm_tc_tile_n(p.N);
-  const int a_box = TC_BM;
-  const int Mp = pad_to(p.M, 128), Np = pad_to(p.N, 128), Kp = pad_to(p.K, BK);
+  const int BK = H ? TcFmt<true>::BK : TcFmt<false>::BK;
+  const TcPlan plan = gemm_tc_plan(p.M, p.N, p.K, p.accumulate, p.split_k, NUM_SMS, H);
+  const int BN = plan.bn;
+  const int a_box = plan.bm;
+  // workspace planes: whole tiles of rows (one tile height, 256, for every plan), K to 128 bytes (the prep kernels' granularity)
+  const int Mp = pad_to(p.M, TC_MPAD), Np = pad_to(p.N, 128), Kp = pad_to(p.K, H ? 2 * TC_KPAD : TC_KPAD);
   int rc;
   // ---- operands: cached planes when the buffer is registered, else a split pass into the shared workspace
   OpView va, vb;
@@ -984,11 +1042,14 @@ int gemm_tc(const AseGemmParams& p, cudaStream_t st, PlaneRegistry* reg) {
   }
   unsigned* oflag = (H && reg) ? reg->flag : nullptr;
   char* wsp = ws + TC_WS_HEAD;
+  // plane slots of the workspace layout.  (They used to be placed at Mp x Kp fp32 words with the FP16 format's K padding to 64,
+  // which for K % 64 in (0, 32] reached past the workspace the caller sized with gemm_tc_workspace_bytes.)
+  const TcWsSlots slots = tc_ws_slots(p.M, p.N, p.K);
   if (va.ok) {
     if ((rc = make_view_map(&ah, va.hi, a_rows, a_cols, va.ldp, p.a_trans ? BK : a_box, p.a_trans != 0, H)) ||
         (rc = make_view_map(&al, va.lo, a_rows, a_cols, va.ldp, p.a_trans ? BK : a_box, p.a_trans != 0, H))) return rc;
   } else {
-    float* Ahi = (float*)wsp; float* Alo = (float*)(wsp + align_up((int64_t)Mp * Kp * 4, 1024));
+    float* Ahi = (float*)wsp; float* Alo = (float*)(wsp + slots.a);
     if (!H) { if ((rc = prep_operand(p.A, p.lda, p.a_trans, p.M, p.K, Mp, Kp, Ahi, Alo, st))) return rc; }
     else {
       if ((rc = materialize_h(p.A, p.lda, a_rows, a_cols, p.a_trans ? Kp : Mp, p.a_trans ? Mp : Kp, Ahi, Alo, t_amax[0], t_scale[0], nullptr, t_pred[0], oflag, st, reg ? TOP_SITE : TOP_EXACT))) return rc;
@@ -1001,8 +1062,8 @@ int gemm_tc(const AseGemmParams& p, cudaStream_t st, PlaneRegistry* reg) {
     if ((rc = make_view_map(&bh, vb.hi, b_rows, b_cols, vb.ldp, p.b_trans ? BK : BN, p.b_trans != 0, H)) ||
         (rc = make_view_map(&bl, vb.lo, b_rows, b_cols, vb.ldp, p.b_trans ? BK : BN, p.b_trans != 0, H))) return rc;
   } else {
-    char* wb = wsp + 2 * align_up((int64_t)Mp * Kp * 4, 1024);
-    float* Bhi = (float*)wb; float* Blo = (float*)(wb + align_up((int64_t)Np * Kp * 4, 1024));
+    char* wb = wsp + 2 * slots.a;
+    float* Bhi = (float*)wb; float* Blo = (float*)(wb + slots.b);
     if (!H) { if ((rc = prep_operand(p.B, p.ldb, p.b_trans, p.N, p.K, Np, Kp, Bhi, Blo, st))) return rc; }
     else {
       if ((rc = materialize_h(p.B, p.ldb, b_rows, b_cols, p.b_trans ? Kp : Np, p.b_trans ? Np : Kp, Bhi, Blo, t_amax[1], t_scale[1], nullptr, t_pred[1], oflag, st, reg ? TOP_SITE : TOP_EXACT))) return rc;
@@ -1057,23 +1118,34 @@ int gemm_tc(const AseGemmParams& p, cudaStream_t st, PlaneRegistry* reg) {
       } else { x->valid = false; x->amax_site = -1; x->is_static = false; }
     }
   }
-  e.kb_total = Kp / BK;
-  { static int dbg = -1; if (dbg < 0) { const char* d = getenv("ASE_TC_DEBUG"); dbg = d ? atoi(d) : 0; } e.debug = dbg; }
-  int splits = (p.accumulate && p.split_k > 1) ? p.split_k : 1;
-  splits = min(splits, e.kb_total);
-  e.kb_per_split = ceil_div(e.kb_total, splits);
-  splits = ceil_div(e.kb_total, e.kb_per_split);
+  e.kb_total = ceil_div(p.K, BK);
+  e.debug = tc_debug();
+  e.kb_per_split = ceil_div(e.kb_total, plan.splits);
+  const int splits = ceil_div(e.kb_total, e.kb_per_split);
   const bool amn = H && p.a_trans, bmn = H && p.b_trans;
-  // 3 stages x 64 KB (128 x 128) / 4 stages x 48 KB (128 x 64) of the 227 KB an H100 block may use
   if (H) {
-    if (BN == 128) return launch_tc_major<128, 3, true>(amn, bmn, ah, al, bh, bl, e, splits, st);
-    return launch_tc_major<64, 4, true>(amn, bmn, ah, al, bh, bl, e, splits, st);
+    if (plan.bm == 256) return BN == 128 ? launch_tc_major<256, 128, true>(amn, bmn, ah, al, bh, bl, e, splits, st)
+                                         : launch_tc_major<256, 64, true>(amn, bmn, ah, al, bh, bl, e, splits, st);
+    return BN == 128 ? launch_tc_major<128, 128, true>(amn, bmn, ah, al, bh, bl, e, splits, st)
+                     : launch_tc_major<128, 64, true>(amn, bmn, ah, al, bh, bl, e, splits, st);
   }
-  if (BN == 128) return launch_tc_major<128, 3, false>(amn, bmn, ah, al, bh, bl, e, splits, st);
-  return launch_tc_major<64, 4, false>(amn, bmn, ah, al, bh, bl, e, splits, st);
+  if (plan.bm == 256) return BN == 128 ? launch_tc_major<256, 128, false>(amn, bmn, ah, al, bh, bl, e, splits, st)
+                                       : launch_tc_major<256, 64, false>(amn, bmn, ah, al, bh, bl, e, splits, st);
+  return BN == 128 ? launch_tc_major<128, 128, false>(amn, bmn, ah, al, bh, bl, e, splits, st)
+                   : launch_tc_major<128, 64, false>(amn, bmn, ah, al, bh, bl, e, splits, st);
 }
 
 }  // namespace ase
+
+extern "C" int ase_gemm_tc_plan(int M, int N, int K, int accumulate, int split_k, int backend, int* tile_m, int* tile_n, int* splits) {
+  using namespace ase;
+  if (M < 1 || N < 1 || K < 1 || (backend != 1 && backend != 2)) { set_error("ase_gemm_tc_plan: bad shape or backend"); return ASE_ERR_INVALID; }
+  const TcPlan p = gemm_tc_plan(M, N, K, accumulate, split_k, NUM_SMS, backend == 2);
+  if (tile_m) *tile_m = p.bm;
+  if (tile_n) *tile_n = p.bn;
+  if (splits) *splits = p.splits;
+  return ASE_OK;
+}
 
 extern "C" int ase_gemm_tc_profile(int enable) {
   ase::g_prof.on = enable != 0;

@@ -82,7 +82,10 @@ struct PlaneRegistry {
 int gemm_tc(const AseGemmParams& p, cudaStream_t st, PlaneRegistry* reg = nullptr);   // wgmma 3xTF32 (backend 1) / 3xFP16-scaled (backend 2) (gemm_tc.cu)
 bool gemm_tc_supported(const AseGemmParams& p);
 int64_t gemm_tc_workspace_bytes(int M, int N, int K);
-int gemm_tc_tile_n(int N);      // N extent of the output tile the tensor-core backends will use for this N
+// tile plan of a tensor-core GEMM (gemm_tc.cu): tile height, tile width, K splits as launched
+struct TcPlan { int bm, bn, splits; };
+constexpr int TC_SPLIT_AUTO = -1;   // split_k for gemm_tc_plan: let the launch-time model choose the splits
+TcPlan gemm_tc_plan(int M, int N, int K, int accumulate, int split_k, int sms, bool f16);
 int gemm_dispatch(const AseGemmParams& p, cudaStream_t st, PlaneRegistry* reg = nullptr);    // picks the backend named in p.backend (falls back to SIMT for shapes tc rejects)
 
 // ------------------------------------------------------------------ loss-side accumulators (doubles)

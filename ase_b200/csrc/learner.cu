@@ -310,8 +310,12 @@ struct G {
     AseGemmParams p = base();
     p.A = dZ; p.lda = ldz; p.a_trans = 1; p.B = X; p.ldb = ldx; p.b_trans = 1; p.C = GR + l.w; p.ldc = l.in;
     p.M = l.out; p.N = l.in; p.K = M; p.accumulate = 1;
-    // split-K so that tiles x splits fills whole waves of the SMs (one CTA each); every extra split adds one RED pass over dW
-    const int tiles = ceil_div(l.out, 128) * ceil_div(l.in, L.cfg.gemm_backend >= 1 ? gemm_tc_tile_n(l.in) : 128);
+    if (L.cfg.gemm_backend >= 1) {      // tile and split-K plan of the tensor-core kernel
+      p.split_k = gemm_tc_plan(p.M, p.N, p.K, 1, TC_SPLIT_AUTO, L.sms, L.cfg.gemm_backend == 2).splits;
+      return gemm_dispatch(p, st, reg());
+    }
+    // SIMT: split-K so that 128 x 128 tiles x splits fill whole waves of the SMs; every extra split adds one RED pass over dW
+    const int tiles = ceil_div(l.out, 128) * ceil_div(l.in, 128);
     const int slots = L.sms;
     const int smax = max(1, min(16, M / 1024));
     int best = 1; double best_cost = 1e30;

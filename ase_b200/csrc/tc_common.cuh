@@ -8,16 +8,15 @@
 
 namespace ase {
 
-constexpr int TC_BM = 128;
-constexpr int TC_BK = 32;                 // fp32 elements per k-block = one 128-byte swizzle row
-constexpr int TC_THREADS = 384;           // warpgroup 0: TMA producer; warpgroups 1, 2: MMA + epilogue, 64 tile rows each
+constexpr int TC_KPAD = 32;               // fp32 words: K padding of workspace planes (128 bytes, the prep kernels' granularity)
+constexpr int TC_THREADS = 384;           // warpgroup 0: TMA producer; warpgroups 1, 2: MMA + epilogue, BM / 2 tile rows each
 
 // Operand-plane formats.  H = false: TF32 hi/lo planes stored as fp32 words (.tf32, K = 8 per MMA, both operands K-major).
 // H = true: SCALED FP16 hi/lo planes (.f16, K = 16 per MMA, twice the MMA rate and half the plane bytes): each tensor is
 // multiplied by a per-tensor power of two that puts its max |x| in [2^8, 2^9) before the split, so hi + lo carries 22
 // significant bits for every element within 2^-22 of the tensor max (absolute floor 2^-25 / scale); the epilogue multiplies
-// by the two inverse scales (exact).  In both formats a k-block is ONE 128-byte swizzle row per operand row, so the shared
-// memory tiles, the TMA transaction bytes and the 4-MMAs-per-k-block structure are identical.
+// by the two inverse scales (exact).  In both formats a k-block is ONE 128-byte swizzle row per operand row (four MMA k-slices),
+// so the shared memory tiles, the TMA transaction bytes and the 12-MMAs-per-k-block-and-m64 structure are identical.
 template <bool H> struct TcFmt {
   static constexpr int BK = H ? 64 : 32;              // elements per k-block (128 bytes)
   // MN-major operands (FP16 planes only)
@@ -25,6 +24,7 @@ template <bool H> struct TcFmt {
   static constexpr int MN_BOX_BYTES = 8192;           // BK k-rows x 128 bytes
   static constexpr int MN_KSTEP = 2048;               // bytes between the MN-major k-slices of consecutive MMAs (16 k-rows)
 };
+constexpr int TC_M64_BYTES = 8192;        // one m64 block of an A plane in both layouts: 64 K-major 128-byte rows / one MN-major box
 
 // ------------------------------------------------------------------------------------------ PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -201,7 +201,8 @@ struct TcEpi {
   const uint32_t* mask_bits; int64_t ldmb; // optional: replaces mask_src for mask_mode 1 (same bit layout)
   int skip_c;                              // the planes are the only consumers of C: no fp32 store
   int debug;   // experiments only (env ASE_TC_DEBUG): 1 skip the whole store phase, 4 skip correction MMAs,
-               // 16 skip mask loads, 32 skip plane stores, 64 skip column-sum atomics, 128 skip the fp32 C store
+               // 16 skip mask loads, 32 skip plane stores, 64 skip column-sum atomics, 128 skip the fp32 C store,
+               // 256 generic store phase only, 512 pin the tile height to 128 rows (gemm_tc_plan)
 };
 
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {

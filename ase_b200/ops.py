@@ -387,6 +387,13 @@ def gemm(A, B, a_trans=False, b_trans=False, bias=None, act=0, mask_src=None, ma
     return out
 
 
+def gemm_tc_plan(M, N, K, accumulate=False, split_k=0, backend=2):
+    """(tile rows, tile cols, K splits) the tensor-core backends launch for this ase_gemm shape (ase_gemm_tc_plan)."""
+    bm, bn, s = C.c_int(), C.c_int(), C.c_int()
+    check(lib.ase_gemm_tc_plan(M, N, K, int(accumulate), split_k, backend, C.byref(bm), C.byref(bn), C.byref(s)), 'ase_gemm_tc_plan')
+    return bm.value, bn.value, s.value
+
+
 # ---- episode resets of HumanoidAMP / HumanoidAMPGetup (env/tasks/humanoid_amp.py:141-246, humanoid_amp_getup.py) -----------------------
 # the YAML constants: humanoid_ase_sword_shield_getup.yaml (ASE pre-training) and humanoid_sword_shield.yaml (AMP)
 STATE_INIT_PARAMS = {

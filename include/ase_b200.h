@@ -330,7 +330,7 @@ typedef struct {
   int act;
   const float* mask_src; int64_t ldm; int mask_mode;
   int accumulate;
-  int split_k;              /* 0/1 = none */
+  int split_k;              /* 0/1 = none; < 0 with accumulate: the tensor-core backends choose (ase_gemm_tc_plan) */
   int backend;
   void* workspace; int64_t workspace_bytes;   /* backends 1, 2: >= ase_gemm_tc_workspace_bytes(), 1024-byte aligned */
   float* colsum_out;        /* optional [N]: colsum_out[n] += sum_m C[m,n] (not with accumulate) */
@@ -345,6 +345,10 @@ typedef struct {
 } AseGemmParams;
 int ase_gemm(const AseGemmParams* p, void* stream);
 int64_t ase_gemm_tc_workspace_bytes(int M, int N, int K);
+/* Tile plan the tensor-core backends (1, 2) use for an ase_gemm of this shape: output tile height (128 or 256) and width
+ * (128 or 64), and the number of K splits as launched.  accumulate and split_k as in AseGemmParams; split_k < 0 (with
+ * accumulate) is the plan the learner uses for its dW GEMMs: the splits are chosen by the kernel's launch-time model. */
+int ase_gemm_tc_plan(int M, int N, int K, int accumulate, int split_k, int backend, int* tile_m, int* tile_n, int* splits);
 /* Live timing of the tensor-core GEMM kernel (bench.py roofline): enable(1)/disable(0) resets the counters; while
  * enabled every launch is bracketed by CUDA events on its stream.  _read synchronises those events and returns the
  * summed kernel time, the launch count and the algorithmic FLOPs (2*M*N*Kpad per launch). */
