@@ -29,7 +29,7 @@ static int check_gemm(const AseGemmParams& p) {
 int gemm_dispatch(const AseGemmParams& p, cudaStream_t st, PlaneRegistry* reg) {
   int rc = check_gemm(p);
   if (rc) return rc;
-  if ((p.backend == 1 || p.backend == 2) && gemm_tc_supported(p)) return gemm_tc(p, st, reg);
+  if (p.backend == 1 || p.backend == 2) return gemm_tc(p, st, reg);
   return gemm_simt(p, st);
 }
 
@@ -43,12 +43,6 @@ extern "C" uint64_t ase_launch_count(void) { return g_launches.load(std::memory_
 
 extern "C" int ase_gemm(const AseGemmParams* p, void* stream) {
   ASE_CHECK_ARG(p != nullptr, "ase_gemm: null params");
-  if (p->backend == 1 || p->backend == 2) {
-    int rc = check_gemm(*p);
-    if (rc) return rc;
-    if (!gemm_tc_supported(*p)) { set_error("ase_gemm: shape %dx%dx%d not supported by the tensor-core backend (needs M>=128, N>=64, K>=32)", p->M, p->N, p->K); return ASE_ERR_UNSUPPORTED; }
-    return gemm_tc(*p, (cudaStream_t)stream);
-  }
   return gemm_dispatch(*p, (cudaStream_t)stream);
 }
 

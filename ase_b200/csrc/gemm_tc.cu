@@ -119,15 +119,7 @@ __device__ __forceinline__ void epilogue_rows(const TcEpi& e, const float* cs, i
     }
     if (e.colsum && !e.accumulate && !(e.debug & 64)) for (int j = 0; j < nvalid; ++j) atomicAdd(s_colsum + cc + j, cs4[j]);   // shared-memory atomics
   }
-  if ((e.c_amax || (H && e.Chi && e.flag)) && !e.accumulate) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
-    if (lane == 0 && amax > 0.0f) {
-      if (e.c_amax) atomicMax(e.c_amax, __float_as_uint(amax));
-      if (H && e.Chi && e.flag && !(amax * cscale <= 60000.0f)) atomicOr(e.flag, 1u);     // the predicted scale was too large: report, never saturate silently
-      if (H && e.Chi && e.flag && cscale == 0.0f) atomicOr(e.flag, 2u);                   // the site only ever saw all-zero tensors, now there is data
-    }
-  }
+  if ((e.c_amax || (H && e.Chi && e.flag)) && !e.accumulate) report_scale_miss(amax, cscale, e.c_amax, (H && e.Chi) ? e.flag : nullptr);
 }
 
 // Fast store phase for interior, aligned tiles of BN = 128 (the generic epilogue_rows above handles everything else).
@@ -260,15 +252,7 @@ __device__ __forceinline__ void epilogue_fast(const TcEpi& e, const float* cs, i
 #pragma unroll
     for (int j = 0; j < CPL; ++j) atomicAdd(s_colsum + c8 + j, csum[j]);
   }
-  if (e.c_amax || (H && e.Chi && e.flag)) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
-    if (lane == 0 && amax > 0.0f) {
-      if (e.c_amax) atomicMax(e.c_amax, __float_as_uint(amax));
-      if (H && e.Chi && e.flag && !(amax * cscale <= 60000.0f)) atomicOr(e.flag, 1u);
-      if (H && e.Chi && e.flag && cscale == 0.0f) atomicOr(e.flag, 2u);
-    }
-  }
+  if (e.c_amax || (H && e.Chi && e.flag)) report_scale_miss(amax, cscale, e.c_amax, (H && e.Chi) ? e.flag : nullptr);
 }
 
 // Ring depth per tile shape: as many stages as fit in ~200 KB of the 227 KB an H100 block may use
@@ -479,109 +463,54 @@ tc_prep_t_kernel(const float* __restrict__ src, int64_t ld, int rows, int cols, 
   }
 }
 
-// FP16 format: max |src| over the [rows, cols] view -> atomicMax on the uint bits (non-negative floats order like uints)
+// FP16 format: max |src| of every item's [rows, cols] view into its amax slot.  blockIdx.y = item, blockIdx.x = slice of it.
+template <int N>
 __global__ void __launch_bounds__(256)
-tc_amax_kernel(const float* __restrict__ src, int64_t ld, int rows, int cols, unsigned* __restrict__ amax) {
-  const int64_t total = (int64_t)rows * cols;
-  float m = 0.0f;
-  if (cols == ld) {
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) m = fmaxf(m, fabsf(src[i]));
-  } else {
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-      const int r = (int)(i / cols), c = (int)(i - (int64_t)r * cols);
-      m = fmaxf(m, fabsf(src[(int64_t)r * ld + c]));
-    }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-  __shared__ float sm[8];
-  if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = m;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int w = 1; w < 8; ++w) m = fmaxf(m, sm[w]);
-    if (m > 0.0f) atomicMax(amax, __float_as_uint(m));
-  }
-}
-
-// FP16 format: split src[rows, cols] (ld) into zero-padded half planes [rows_p, cols_p]; 4 consecutive columns per thread
-// (cols_p is a multiple of 8).  Two modes, both without a host sync:
-//   amax_in != null : EXACT  -- the scale is derived from the tensor's max (already in device memory) and published with its
-//                              inverse in scale_io[0..1] for the epilogues of the GEMMs that consume these planes;
-//   amax_in == null : PREDICTED -- scale_io holds the scale derived from the previous call's max at this site; this pass tracks
-//                              the current max into amax_out for the next call and raises flag bit 0 if a value does not fit.
-__global__ void __launch_bounds__(256)
-tc_prep_h_kernel(const float* __restrict__ src, int64_t ld, int rows, int cols, int rows_p, int cols_p, __half* __restrict__ hi,
-                 __half* __restrict__ lo, const unsigned* __restrict__ amax_in, float* __restrict__ scale_io, float* __restrict__ scale_copy,
-                 unsigned* __restrict__ amax_out, unsigned* __restrict__ flag, int top) {
-  float s;
-  if (amax_in) {
-    s = scale_from_amax(__uint_as_float(*amax_in), top);
-    if (blockIdx.x == 0 && threadIdx.x == 0) { scale_io[0] = s; scale_io[1] = 1.0f / s; }
-  } else s = scale_io[0];
-  if (scale_copy && blockIdx.x == 0 && threadIdx.x == 0) { scale_copy[0] = s; scale_copy[1] = (s != 0.0f) ? 1.0f / s : 0.0f; }
-  const int c4n = cols_p >> 2;
-  const int64_t total = (int64_t)rows_p * c4n;
-  const bool vec = ((ld & 3) == 0) && ((reinterpret_cast<uintptr_t>(src) & 15) == 0);
-  float m = 0.0f;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    const int r = (int)(i / c4n), c = (int)(i - (int64_t)r * c4n) * 4;
-    float x[4] = {0.0f, 0.0f, 0.0f, 0.0f};
-    if (r < rows) {
-      const float* sp = src + (int64_t)r * ld + c;
-      if (vec && c + 4 <= cols) { const float4 t = *reinterpret_cast<const float4*>(sp); x[0] = t.x; x[1] = t.y; x[2] = t.z; x[3] = t.w; }
-      else for (int j = 0; j < 4; ++j) if (c + j < cols) x[j] = sp[j];
-    }
-#pragma unroll
-    for (int j = 0; j < 4; ++j) m = fmaxf(m, fabsf(x[j]));
-    uint2 hv, lv;
-    split_f16x2(x[0] * s, x[1] * s, hv.x, lv.x); split_f16x2(x[2] * s, x[3] * s, hv.y, lv.y);
-    *reinterpret_cast<uint2*>(hi + (int64_t)r * cols_p + c) = hv;
-    *reinterpret_cast<uint2*>(lo + (int64_t)r * cols_p + c) = lv;
-  }
-  if (!amax_in) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if ((threadIdx.x & 31) == 0 && m > 0.0f) {
-      if (amax_out) atomicMax(amax_out, __float_as_uint(m));
-      if (flag && !(m * s <= 60000.0f)) atomicOr(flag, 1u);
-      if (flag && s == 0.0f) atomicOr(flag, 2u);       // the site only ever saw an all-zero tensor, now there is data
-    }
-  }
-}
-
-// FP16 format: all weight tensors of the learner in ONE launch (they are re-split after every optimizer step; one launch
-// per tensor cost ~7 us each for a few MB of work).  blockIdx.y = tensor, blockIdx.x = slice of it.
-__global__ void __launch_bounds__(256)
-tc_amax_batch_kernel(TcPrepBatch b, unsigned* __restrict__ amax) {
-  const TcPrepItem it = b.item[blockIdx.y];
+tc_amax_kernel(const TcPrepList<N> l) {
+  const TcPrepItem it = l.item[blockIdx.y];
   const int64_t total = (int64_t)it.rows * it.cols;
   float m = 0.0f;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) m = fmaxf(m, fabsf(it.src[i]));
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-  if ((threadIdx.x & 31) == 0 && m > 0.0f) atomicMax(amax + it.site, __float_as_uint(m));
+  if (it.cols == it.ld) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) m = fmaxf(m, fabsf(it.src[i]));
+  } else {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+      const int r = (int)(i / it.cols), c = (int)(i - (int64_t)r * it.cols);
+      m = fmaxf(m, fabsf(it.src[(int64_t)r * it.ld + c]));
+    }
+  }
+  report_scale_miss(m, 1.0f, it.amax, nullptr);      // no flag: the max only
 }
+
+// FP16 format: split every item into its half planes, 4 consecutive columns per thread (ldp is a multiple of 8); blockIdx.y = item,
+// blockIdx.x = slice of it.  Two modes, both without a host sync:
+//   exact     : the scale is derived from the max already in the item's amax slot and published with its inverse in scale[0..1]
+//               for the epilogues of the GEMMs that consume these planes;
+//   predicted : scale[0] holds the scale derived from the previous call's max at this site; this pass tracks the current max into
+//               the amax slot for the next call and reports a scale miss in `flag`.
+// scale_copy, if set, receives the scale and its inverse (0 for a zero scale): a copy that outlives the site's slot.
+template <int N>
 __global__ void __launch_bounds__(256)
-tc_prep_h_batch_kernel(TcPrepBatch b, unsigned* __restrict__ amax, float* __restrict__ scale, float* __restrict__ bscale, int exact,
-                       unsigned* __restrict__ flag) {
-  const TcPrepItem it = b.item[blockIdx.y];
+tc_split_h_kernel(const TcPrepList<N> l, int exact, int top, unsigned* __restrict__ flag) {
+  const TcPrepItem it = l.item[blockIdx.y];
   float s;
   if (exact) {
-    s = scale_from_amax(__uint_as_float(amax[it.site]), TOP_SITE);
-    if (blockIdx.x == 0 && threadIdx.x == 0) { scale[2 * it.site] = s; scale[2 * it.site + 1] = 1.0f / s; }
-  } else s = scale[2 * it.site];
-  if (blockIdx.x == 0 && threadIdx.x == 0) { bscale[2 * it.buf] = s; bscale[2 * it.buf + 1] = (s != 0.0f) ? 1.0f / s : 0.0f; }
+    s = scale_from_amax(__uint_as_float(*it.amax), top);
+    if (blockIdx.x == 0 && threadIdx.x == 0) { it.scale[0] = s; it.scale[1] = 1.0f / s; }
+  } else s = it.scale[0];
+  if (it.scale_copy && blockIdx.x == 0 && threadIdx.x == 0) { it.scale_copy[0] = s; it.scale_copy[1] = (s != 0.0f) ? 1.0f / s : 0.0f; }
   __half* hi = (__half*)it.hi; __half* lo = (__half*)it.lo;
   const int c4n = it.ldp >> 2;
-  const int64_t total = (int64_t)it.rows * c4n;
-  const bool vec = (it.cols & 3) == 0;         // weight rows are contiguous (ld = cols) and the arena offsets 128-byte aligned
+  const int64_t total = (int64_t)it.rows_p * c4n;
+  const bool vec = ((it.ld & 3) == 0) && ((reinterpret_cast<uintptr_t>(it.src) & 15) == 0);
   float m = 0.0f;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int r = (int)(i / c4n), c = (int)(i - (int64_t)r * c4n) * 4;
     float x[4] = {0.0f, 0.0f, 0.0f, 0.0f};
-    const float* sp = it.src + (int64_t)r * it.cols + c;
-    if (vec && c + 4 <= it.cols) { const float4 t = *reinterpret_cast<const float4*>(sp); x[0] = t.x; x[1] = t.y; x[2] = t.z; x[3] = t.w; }
-    else for (int j = 0; j < 4; ++j) if (c + j < it.cols) x[j] = sp[j];
+    if (r < it.rows) {
+      const float* sp = it.src + (int64_t)r * it.ld + c;
+      if (vec && c + 4 <= it.cols) { const float4 t = *reinterpret_cast<const float4*>(sp); x[0] = t.x; x[1] = t.y; x[2] = t.z; x[3] = t.w; }
+      else for (int j = 0; j < 4; ++j) if (c + j < it.cols) x[j] = sp[j];
+    }
 #pragma unroll
     for (int j = 0; j < 4; ++j) m = fmaxf(m, fabsf(x[j]));
     uint2 hv, lv;
@@ -589,15 +518,7 @@ tc_prep_h_batch_kernel(TcPrepBatch b, unsigned* __restrict__ amax, float* __rest
     *reinterpret_cast<uint2*>(hi + (int64_t)r * it.ldp + c) = hv;
     *reinterpret_cast<uint2*>(lo + (int64_t)r * it.ldp + c) = lv;
   }
-  if (!exact) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if ((threadIdx.x & 31) == 0 && m > 0.0f) {
-      atomicMax(amax + it.site, __float_as_uint(m));
-      if (!(m * s <= 60000.0f)) atomicOr(flag, 1u);
-      if (s == 0.0f) atomicOr(flag, 2u);
-    }
-  }
+  if (!exact) report_scale_miss(m, s, it.amax, flag);
 }
 
 // FP16 format, start of every top-level call: fold the maxima tracked during the previous call into the sites' scales (the
@@ -654,7 +575,7 @@ static std::unordered_map<MapKey, CUtensorMap, MapKeyHash>& map_cache() { static
 
 // 2D map over [rows, cols] elements (cols contiguous, row stride ld elements); the box is one 128-byte row chunk
 // (32 fp32 words / 64 halfs) x box_rows, 128-byte swizzle
-static int encode_cached(CUtensorMap* tm, const void* base, int rows, int cols, int64_t ld, int box_rows, bool mn_major, bool half = false) {
+static int encode_cached(CUtensorMap* tm, const void* base, int rows, int cols, int64_t ld, int box_rows, bool mn_major, bool half) {
   MapKey k{base, rows, cols, ld, box_rows, (mn_major ? 1 : 0) | (half ? 2 : 0)};
   auto& c = map_cache();
   auto it = c.find(k);
@@ -675,11 +596,6 @@ static int encode_cached(CUtensorMap* tm, const void* base, int rows, int cols, 
   return ASE_OK;
 }
 
-// 2D tensor map over a zero-padded plane [rows_p, cols_p] (cols contiguous)
-static int make_map(CUtensorMap* tm, const void* base, int rows_p, int cols_p, int box_rows, bool mn_major = false, bool half = false) {
-  return encode_cached(tm, base, rows_p, cols_p, cols_p, box_rows, mn_major, half);
-}
-
 static inline int pad_to(int x, int m) { return (x + m - 1) / m * m; }
 
 // planes are padded to whole tiles in both dimensions (zero filled by the prep kernel), M to the tallest tile (256 rows)
@@ -698,9 +614,6 @@ int64_t gemm_tc_workspace_bytes(int M, int N, int K) {
   const TcWsSlots s = tc_ws_slots(M, N, K);
   return TC_WS_HEAD + 2 * s.a + 2 * s.b;
 }
-
-// every shape runs on the tensor cores (small heads are padded up to one tile)
-bool gemm_tc_supported(const AseGemmParams& p) { return p.M >= 1 && p.N >= 1 && p.K >= 1; }
 
 // a missing / small / misaligned workspace is an ERROR, never a silent fallback
 int gemm_tc_check_workspace(const AseGemmParams& p) {
@@ -726,28 +639,20 @@ static int prep_operand(const float* src, int64_t ld, int trans, int rows, int K
   return ASE_OK;
 }
 
-static int launch_amax(const float* src, int64_t ld, int rows, int cols, unsigned* amax, cudaStream_t st) {
-  const int64_t total = (int64_t)rows * cols;
-  tc_amax_kernel<<<(int)imin64((total + 1023) / 1024, NUM_SMS * 8), 256, 0, st>>>(src, ld, rows, cols, amax);
+// FP16 format: split one tensor into half planes.  With a predicted scale (scale_known: the site's scale from the previous call)
+// one pass also tracks the tensor's max for the next call.  Else the scale is exact, from the max in it.amax, which a max pass
+// computes first unless max_known (the GEMM that wrote the tensor tracked it).
+static int materialize_h(const TcPrepItem& it, bool scale_known, bool max_known, unsigned* flag, int top, cudaStream_t st) {
+  const TcPrepList<1> l{{it}};
+  if (!scale_known && !max_known) {
+    const int64_t total = (int64_t)it.rows * it.cols;
+    tc_amax_kernel<1><<<(int)imin64((total + 1023) / 1024, NUM_SMS * 8), 256, 0, st>>>(l);
+    ASE_LAUNCH_OK();
+  }
+  const int64_t total = (int64_t)it.rows_p * (it.ldp / 4);
+  tc_split_h_kernel<1><<<(int)imin64((total + 255) / 256, NUM_SMS * 16), 256, 0, st>>>(l, scale_known ? 0 : 1, top, flag);
   ASE_LAUNCH_OK();
   return ASE_OK;
-}
-static int launch_prep_h(const float* src, int64_t ld, int rows, int cols, int rows_p, int cols_p, void* hi, void* lo, const unsigned* amax_in,
-                         float* scale_io, float* scale_copy, unsigned* amax_out, unsigned* flag, cudaStream_t st, int top = TOP_SITE) {
-  const int64_t total = (int64_t)rows_p * (cols_p / 4);
-  tc_prep_h_kernel<<<(int)imin64((total + 255) / 256, NUM_SMS * 16), 256, 0, st>>>(src, ld, rows, cols, rows_p, cols_p, (__half*)hi, (__half*)lo, amax_in,
-                                                                              scale_io, scale_copy, amax_out, flag, top);
-  ASE_LAUNCH_OK();
-  return ASE_OK;
-}
-// FP16 format: materialise the planes of a tensor nobody split yet.  predicted: the site's scale from the previous call is used
-// (one pass); else a max pass runs first (two passes, exact scale).
-static int materialize_h(const float* src, int64_t ld, int sr, int sc, int pr, int pc, void* hi, void* lo, unsigned* amax, float* scale,
-                         float* scale_copy, bool predicted, unsigned* flag, cudaStream_t st, int top = TOP_SITE) {
-  if (predicted) return launch_prep_h(src, ld, sr, sc, pr, pc, hi, lo, nullptr, scale, scale_copy, amax, flag, st);
-  int rc;
-  if ((rc = launch_amax(src, ld, sr, sc, amax, st))) return rc;
-  return launch_prep_h(src, ld, sr, sc, pr, pc, hi, lo, amax, scale, scale_copy, nullptr, nullptr, st, top);
 }
 
 // Optional per-launch timing of the main kernel (bench.py's live roofline measurement): CUDA events recorded on
@@ -769,11 +674,7 @@ static void prof_mark(cudaStream_t st) {
   cudaEventRecord(g_prof.ev[g_prof.used++], st);
 }
 
-bool tc_prof_on() { return g_prof.on; }
-void tc_prof_mark(cudaStream_t st) { prof_mark(st); }
-void tc_prof_add_flops(double f) { g_prof.flops += f; }
-
-int tc_pdl() {   // env ASE_TC_PDL=0 launches the GEMMs fully stream-serialised
+static int tc_pdl() {   // env ASE_TC_PDL=0 launches the GEMMs fully stream-serialised
   static int v = -1;
   if (v < 0) { const char* d = getenv("ASE_TC_PDL"); v = d ? (atoi(d) != 0) : 1; }
   return v;
@@ -867,14 +768,14 @@ void PlaneRegistry::add(const float* base, int64_t capacity, float* hi, float* l
   if (n >= MAX) return;
   PlaneBuf& x = b[n++];
   x.base = base; x.capacity = capacity; x.hi = hi; x.lo = lo; x.plane_capacity = plane_capacity;
-  x.ld = 0; x.rows = x.cols = 0; x.ldp = 0; x.valid = false; x.scale_ptr = nullptr; x.amax_site = -1; x.is_static = false; x.fp32_stale = false;
+  x.ld = 0; x.rows = x.cols = 0; x.ldp = 0; x.scale_ptr = nullptr; x.drop();
 }
 PlaneBuf* PlaneRegistry::declare(const float* base, int64_t ld, int rows, int cols) {
   PlaneBuf* x = find(base);
   if (!x || x->base != base) return nullptr;
-  x->amax_site = -1; x->is_static = false; x->fp32_stale = false;
+  x->drop();
   const int64_t ldp = f16 ? (cols + 7) / 8 * 8 : (cols + 3) / 4 * 4;
-  if ((int64_t)rows * ldp > (f16 ? 2 : 1) * x->plane_capacity) { x->valid = false; return nullptr; }
+  if ((int64_t)rows * ldp > (f16 ? 2 : 1) * x->plane_capacity) return nullptr;
   x->ld = ld; x->rows = rows; x->cols = cols; x->ldp = ldp; x->valid = true;
   if (f16) { x->is_static = true; x->scale_ptr = static_scale; }
   return x;
@@ -884,9 +785,9 @@ void* PlaneRegistry::plane(const PlaneBuf* x, bool lo, int64_t r0, int64_t c0) c
   const int64_t off = r0 * x->ldp + c0;
   return f16 ? (void*)((__half*)p + off) : (void*)(p + off);
 }
-void PlaneRegistry::invalidate(const float* p) { if (PlaneBuf* x = find(p)) { x->valid = false; x->amax_site = -1; x->is_static = false; x->fp32_stale = false; } }
+void PlaneRegistry::invalidate(const float* p) { if (PlaneBuf* x = find(p)) x->drop(); }
 void PlaneRegistry::invalidate_range(const float* lo_, const float* hi_) {
-  for (int i = 0; i < n; ++i) if (b[i].base >= lo_ && b[i].base < hi_) { b[i].valid = false; b[i].amax_site = -1; b[i].is_static = false; b[i].fp32_stale = false; }
+  for (int i = 0; i < n; ++i) if (b[i].base >= lo_ && b[i].base < hi_) b[i].drop();
 }
 int PlaneRegistry::begin_call(cudaStream_t st, int base) {
   call_base = base; gemm_index = 0;
@@ -920,20 +821,19 @@ int PlaneRegistry::prep_weights(const float* const* src, const int* rows, const 
     if ((int64_t)rows[i] * ldp > 2 * x->plane_capacity) continue;
     const int site = WEIGHT_SITE0 + i;
     if (site >= SITES) break;
-    TcPrepItem& it = batch.item[nb++];
-    it.src = src[i]; it.hi = x->hi; it.lo = x->lo; it.rows = rows[i]; it.cols = cols[i]; it.ldp = (int)ldp; it.site = site; it.buf = (int)(x - b);
     x->ld = cols[i]; x->rows = rows[i]; x->cols = cols[i]; x->ldp = ldp; x->valid = true; x->is_static = false; x->amax_site = -1; x->fp32_stale = false;
-    x->scale_ptr = bscale + 2 * it.buf;
+    x->scale_ptr = bscale + 2 * (x - b);
+    batch.item[nb++] = {src[i], cols[i], rows[i], cols[i], rows[i], (int)ldp, x->hi, x->lo, amax + site, scale + 2 * site, bscale + 2 * (x - b)};
     all_known = all_known && known[site];
     touched[site] = true;
   }
   if (nb == 0) return ASE_OK;
   dim3 grid(48, nb);      // 28 MB of weights per optimizer step: 48 slices x 16 tensors keep every SM several blocks deep
   if (!all_known) {
-    tc_amax_batch_kernel<<<grid, 256, 0, st>>>(batch, amax);
+    tc_amax_kernel<<<grid, 256, 0, st>>>(batch);
     ASE_LAUNCH_OK();
   }
-  tc_prep_h_batch_kernel<<<grid, 256, 0, st>>>(batch, amax, scale, bscale, all_known ? 0 : 1, flag);
+  tc_split_h_kernel<<<grid, 256, 0, st>>>(batch, all_known ? 0 : 1, TOP_SITE, flag);
   ASE_LAUNCH_OK();
   return ASE_OK;
 }
@@ -968,14 +868,15 @@ static int resolve_operand(PlaneRegistry* reg, const float* ptr, int64_t ld, int
         // written earlier in this call by a GEMM whose scale was not known yet: it declared the geometry and tracked max |C|
         const int ts = x->amax_site;
         x->ldp = pad_to(x->cols, 8);
-        if ((rc = launch_prep_h(ptr, x->ld, x->rows, x->cols, x->rows, (int)x->ldp, x->hi, x->lo, reg->amax + ts, reg->scale + 2 * ts, bs, nullptr, nullptr, st))) return rc;
+        const TcPrepItem it{ptr, x->ld, x->rows, x->cols, x->rows, (int)x->ldp, x->hi, x->lo, reg->amax + ts, reg->scale + 2 * ts, bs};
+        if ((rc = materialize_h(it, false, true, nullptr, TOP_SITE, st))) return rc;
       } else {
         // written by a non-GEMM kernel (or accumulated into): split the reader's view with this reader's site
         const int64_t ldp = pad_to(nat_cols, 8);
         if (site < 0 || (int64_t)nat_rows * ldp > 2 * x->plane_capacity || (int64_t)(nat_rows - 1) * ld + nat_cols > x->capacity) return ASE_OK;
         x->ld = ld; x->rows = nat_rows; x->cols = nat_cols; x->ldp = ldp;
-        if ((rc = materialize_h(ptr, ld, nat_rows, nat_cols, nat_rows, (int)ldp, x->hi, x->lo, reg->amax + site, reg->scale + 2 * site, bs, reg->known[site],
-                                reg->flag, st))) return rc;
+        const TcPrepItem it{ptr, ld, nat_rows, nat_cols, nat_rows, (int)ldp, x->hi, x->lo, reg->amax + site, reg->scale + 2 * site, bs};
+        if ((rc = materialize_h(it, reg->known[site], false, reg->flag, TOP_SITE, st))) return rc;
         reg->touched[site] = true;
       }
       x->scale_ptr = bs; x->is_static = false;
@@ -990,11 +891,6 @@ static int resolve_operand(PlaneRegistry* reg, const float* ptr, int64_t ld, int
   if (H) v->scale = x->scale_ptr;
   v->ldp = x->ldp; v->ok = true;
   return ASE_OK;
-}
-
-// tensor map over a (sub-)view of a plane with TRUE extents: TMA zero-fills everything outside [rows, cols]
-static int make_view_map(CUtensorMap* tm, const void* base, int rows, int cols, int64_t ldp, int box_rows, bool mn_major, bool half) {
-  return encode_cached(tm, base, rows, cols, ldp, box_rows, mn_major, half);
 }
 
 int gemm_tc(const AseGemmParams& p, cudaStream_t st, PlaneRegistry* reg) {
@@ -1046,31 +942,34 @@ int gemm_tc(const AseGemmParams& p, cudaStream_t st, PlaneRegistry* reg) {
   // which for K % 64 in (0, 32] reached past the workspace the caller sized with gemm_tc_workspace_bytes.)
   const TcWsSlots slots = tc_ws_slots(p.M, p.N, p.K);
   if (va.ok) {
-    if ((rc = make_view_map(&ah, va.hi, a_rows, a_cols, va.ldp, p.a_trans ? BK : a_box, p.a_trans != 0, H)) ||
-        (rc = make_view_map(&al, va.lo, a_rows, a_cols, va.ldp, p.a_trans ? BK : a_box, p.a_trans != 0, H))) return rc;
+    // TRUE extents over a (sub-)view of the planes: TMA zero-fills everything outside [a_rows, a_cols]
+    if ((rc = encode_cached(&ah, va.hi, a_rows, a_cols, va.ldp, p.a_trans ? BK : a_box, p.a_trans != 0, H)) ||
+        (rc = encode_cached(&al, va.lo, a_rows, a_cols, va.ldp, p.a_trans ? BK : a_box, p.a_trans != 0, H))) return rc;
   } else {
     float* Ahi = (float*)wsp; float* Alo = (float*)(wsp + slots.a);
     if (!H) { if ((rc = prep_operand(p.A, p.lda, p.a_trans, p.M, p.K, Mp, Kp, Ahi, Alo, st))) return rc; }
     else {
-      if ((rc = materialize_h(p.A, p.lda, a_rows, a_cols, p.a_trans ? Kp : Mp, p.a_trans ? Mp : Kp, Ahi, Alo, t_amax[0], t_scale[0], nullptr, t_pred[0], oflag, st, reg ? TOP_SITE : TOP_EXACT))) return rc;
+      const TcPrepItem it{p.A, p.lda, a_rows, a_cols, p.a_trans ? Kp : Mp, p.a_trans ? Mp : Kp, Ahi, Alo, t_amax[0], t_scale[0], nullptr};
+      if ((rc = materialize_h(it, t_pred[0], false, oflag, reg ? TOP_SITE : TOP_EXACT, st))) return rc;
       va.scale = t_scale[0];
     }
-    if (!p.a_trans || !H) { if ((rc = make_map(&ah, Ahi, Mp, Kp, a_box, false, H)) || (rc = make_map(&al, Alo, Mp, Kp, a_box, false, H))) return rc; }
-    else            { if ((rc = make_map(&ah, Ahi, Kp, Mp, BK, true, H)) || (rc = make_map(&al, Alo, Kp, Mp, BK, true, H))) return rc; }
+    if (!p.a_trans || !H) { if ((rc = encode_cached(&ah, Ahi, Mp, Kp, Kp, a_box, false, H)) || (rc = encode_cached(&al, Alo, Mp, Kp, Kp, a_box, false, H))) return rc; }
+    else            { if ((rc = encode_cached(&ah, Ahi, Kp, Mp, Mp, BK, true, H)) || (rc = encode_cached(&al, Alo, Kp, Mp, Mp, BK, true, H))) return rc; }
   }
   if (vb.ok) {
-    if ((rc = make_view_map(&bh, vb.hi, b_rows, b_cols, vb.ldp, p.b_trans ? BK : BN, p.b_trans != 0, H)) ||
-        (rc = make_view_map(&bl, vb.lo, b_rows, b_cols, vb.ldp, p.b_trans ? BK : BN, p.b_trans != 0, H))) return rc;
+    if ((rc = encode_cached(&bh, vb.hi, b_rows, b_cols, vb.ldp, p.b_trans ? BK : BN, p.b_trans != 0, H)) ||
+        (rc = encode_cached(&bl, vb.lo, b_rows, b_cols, vb.ldp, p.b_trans ? BK : BN, p.b_trans != 0, H))) return rc;
   } else {
     char* wb = wsp + 2 * slots.a;
     float* Bhi = (float*)wb; float* Blo = (float*)(wb + slots.b);
     if (!H) { if ((rc = prep_operand(p.B, p.ldb, p.b_trans, p.N, p.K, Np, Kp, Bhi, Blo, st))) return rc; }
     else {
-      if ((rc = materialize_h(p.B, p.ldb, b_rows, b_cols, p.b_trans ? Kp : Np, p.b_trans ? Np : Kp, Bhi, Blo, t_amax[1], t_scale[1], nullptr, t_pred[1], oflag, st, reg ? TOP_SITE : TOP_EXACT))) return rc;
+      const TcPrepItem it{p.B, p.ldb, b_rows, b_cols, p.b_trans ? Kp : Np, p.b_trans ? Np : Kp, Bhi, Blo, t_amax[1], t_scale[1], nullptr};
+      if ((rc = materialize_h(it, t_pred[1], false, oflag, reg ? TOP_SITE : TOP_EXACT, st))) return rc;
       vb.scale = t_scale[1];
     }
-    if (!p.b_trans || !H) { if ((rc = make_map(&bh, Bhi, Np, Kp, BN, false, H)) || (rc = make_map(&bl, Blo, Np, Kp, BN, false, H))) return rc; }
-    else            { if ((rc = make_map(&bh, Bhi, Kp, Np, BK, true, H)) || (rc = make_map(&bl, Blo, Kp, Np, BK, true, H))) return rc; }
+    if (!p.b_trans || !H) { if ((rc = encode_cached(&bh, Bhi, Np, Kp, Kp, BN, false, H)) || (rc = encode_cached(&bl, Blo, Np, Kp, Kp, BN, false, H))) return rc; }
+    else            { if ((rc = encode_cached(&bh, Bhi, Kp, Np, Np, BK, true, H)) || (rc = encode_cached(&bl, Blo, Kp, Np, Np, BK, true, H))) return rc; }
   }
   TcEpi e;
   e.C = p.C; e.ldc = p.ldc; e.M = p.M; e.N = p.N; e.K = p.K; e.alpha = p.alpha; e.bias = p.bias; e.act = p.act;
@@ -1114,8 +1013,8 @@ int gemm_tc(const AseGemmParams& p, cudaStream_t st, PlaneRegistry* reg) {
       } else if (!p.accumulate && x->valid && x->is_static && x->ld == p.ldc && p.act == 2 && !p.mask_src) {
         const int64_t off = p.C - x->base, r0 = off / x->ld, c0 = off - r0 * x->ld;
         if (r0 + p.M <= x->rows && c0 + p.N <= x->cols) { e.Chi = reg->plane(x, false, r0, c0); e.Clo = reg->plane(x, true, r0, c0); e.ldp = x->ldp; e.c_scale = x->scale_ptr; e.flag = reg->flag; }
-        else { x->valid = false; x->amax_site = -1; x->is_static = false; }
-      } else { x->valid = false; x->amax_site = -1; x->is_static = false; }
+        else x->drop();
+      } else x->drop();
     }
   }
   e.kb_total = ceil_div(p.K, BK);

@@ -33,6 +33,7 @@ struct PlaneBuf {
   int amax_site;                                // site whose amax slot holds max |x| of the current fp32 contents (tracked by the GEMM that wrote them), -1 = unknown
   bool is_static;                               // planes written with the registry's static scale by a bounded non-GEMM writer
   bool fp32_stale;                              // the last producer skipped the fp32 store (c_planes_only): only the planes are current
+  void drop() { valid = false; amax_site = -1; is_static = false; fp32_stale = false; }   // the buffer has no current planes
 };
 // FP16 format (backend 2): every tensor is multiplied by a power of two before the hi/lo split.  Scales live in device memory,
 // one slot per SITE = (GEMM index within the top-level call, operand A / B / output C): the static kernel schedule of the learner
@@ -43,8 +44,15 @@ struct PlaneBuf {
 // the same call.  Underflow: a scaled max below 2^-6, i.e. shrinking by more than 2^14 .. 2^15 (never flagged at 2^-13, always at
 // 2^-16), is flagged by tc_site_update_kernel at the start of the NEXT call.  Either raises a sticky device flag
 // (ase_learner_plane_status), never a silent wrong result (tests/test_gpu_learner_shapes.py pins both edges).
-struct TcPrepItem { const float* src; void* hi; void* lo; int rows, cols, ldp, site, buf; };
-struct TcPrepBatch { static constexpr int MAX = 40; TcPrepItem item[MAX]; };
+// One tensor for the FP16 split pass: src[rows, cols] (ld) into zero-padded planes [rows_p, ldp]; its max slot, its site's
+// [scale, 1/scale] and an optional copy of the scale the planes are written with.
+struct TcPrepItem {
+  const float* src; int64_t ld; int rows, cols, rows_p, ldp;
+  void* hi; void* lo;
+  unsigned* amax; float* scale; float* scale_copy;
+};
+template <int N> struct TcPrepList { static constexpr int MAX = N; TcPrepItem item[N]; };
+using TcPrepBatch = TcPrepList<40>;   // the learner's weight tensors, split in one launch
 struct PlaneRegistry {
   static constexpr int MAX = 160;
   static constexpr int WEIGHT_SITE0 = 960;      // fixed scale sites of the weight tensors (prep_weights)
@@ -80,13 +88,12 @@ struct PlaneRegistry {
   void invalidate_range(const float* lo_, const float* hi_);
 };
 int gemm_tc(const AseGemmParams& p, cudaStream_t st, PlaneRegistry* reg = nullptr);   // wgmma 3xTF32 (backend 1) / 3xFP16-scaled (backend 2) (gemm_tc.cu)
-bool gemm_tc_supported(const AseGemmParams& p);
 int64_t gemm_tc_workspace_bytes(int M, int N, int K);
 // tile plan of a tensor-core GEMM (gemm_tc.cu): tile height, tile width, K splits as launched
 struct TcPlan { int bm, bn, splits; };
 constexpr int TC_SPLIT_AUTO = -1;   // split_k for gemm_tc_plan: let the launch-time model choose the splits
 TcPlan gemm_tc_plan(int M, int N, int K, int accumulate, int split_k, int sms, bool f16);
-int gemm_dispatch(const AseGemmParams& p, cudaStream_t st, PlaneRegistry* reg = nullptr);    // picks the backend named in p.backend (falls back to SIMT for shapes tc rejects)
+int gemm_dispatch(const AseGemmParams& p, cudaStream_t st, PlaneRegistry* reg = nullptr);    // checks p and runs the backend it names
 
 // ------------------------------------------------------------------ loss-side accumulators (doubles)
 enum {

@@ -80,6 +80,7 @@ struct AseLearner {
   int B, Ba, Ra;            // Ra = actor rows (2B when the diversity pass is batched in)
   int sms;                  // SMs of the device the learner was created on (split-K planning of the dW GEMMs)
   int in0, ldx, amp_ld, maxw;
+  int64_t gsz;              // floats of each gradient scratch buffer G0, G1
   // workspace
   float *Xa, *Xc, *Zc, *S[ASE_MAX_LAYERS], *H[ASE_MAX_LAYERS], *MU, *C[ASE_MAX_LAYERS], *V;
   float *Xd, *D[ASE_MAX_LAYERS], *LOGIT, *E;
@@ -135,6 +136,31 @@ static int64_t tc_ws_need(const AseLearner& L) {
   return need;
 }
 
+// Every buffer with operand planes on the tensor-core backends, as f(fp32 base, rows, cols, is_weight): the activation buffers, then
+// every tensor of the parameter arena at `params` (null: base pointers not needed).  carve() sizes the plane regions with it and
+// register_planes() registers the same list.
+template <typename F>
+static void for_each_plane_buf(const AseLearner& L, const float* params, F&& f) {
+  const AseLearnerConfig& c = L.cfg;
+  const int64_t Ra = L.Ra, B = L.B, Ba = L.Ba;
+  f(L.Xa, Ra, L.ldx, false);
+  if (L.ase) { f(L.Xc, B, L.ldx, false); f(L.Zc, Ra, c.latent_dim, false); for (int k = 0; k < c.n_style_units; ++k) f(L.S[k], Ra, c.style_units[k], false); }
+  for (int k = 0; k < c.n_units; ++k) { f(L.H[k], Ra, c.units[k], false); f(L.C[k], B, c.units[k], false); }
+  if (L.amp) {
+    f(L.Xd, 3 * Ba, L.amp_ld, false);
+    for (int k = 0; k < c.n_disc_units; ++k) { f(L.D[k], 3 * Ba, c.disc_units[k], false); f(L.U[k], Ba, c.disc_units[k], false); }
+    f(L.Gx, Ba, L.amp_ld, false);
+  }
+  f(L.G0, 1, L.gsz, false); f(L.G1, 1, L.gsz, false);
+  // head gradients (written by the loss kernels): split once for their dW and dX consumers
+  f(L.dMU, Ra, c.act_dim, false); f(L.dV, B, 1, false);
+  if (L.amp) { f(L.dLOGIT, 3 * Ba, 1, false); if (L.ase) f(L.dE, Ba, c.latent_dim, false); }
+  for (int i = 0; i < L.net.n_tensors; ++i) {
+    const TensorDesc& d = L.net.desc[i];
+    f(params ? params + d.off : nullptr, d.rows, d.cols, true);
+  }
+}
+
 static void carve(AseLearner& L, void* ws, int64_t* total) {
   const AseLearnerConfig& c = L.cfg;
   Carver cv(ws);
@@ -149,7 +175,6 @@ static void carve(AseLearner& L, void* ws, int64_t* total) {
   L.V = cv.take<float>(B);
   L.dMU = cv.take<float>(Ra * c.act_dim);
   L.dV = cv.take<float>(B);
-  int64_t gsz = Ra * (int64_t)L.maxw;
   if (L.amp) {
     L.Xd = cv.take<float>(3 * Ba * L.amp_ld);
     for (int k = 0; k < c.n_disc_units; ++k) L.D[k] = cv.take<float>(3 * Ba * c.disc_units[k]);
@@ -158,12 +183,9 @@ static void carve(AseLearner& L, void* ws, int64_t* total) {
     if (L.ase) { L.E = cv.take<float>(3 * Ba * c.latent_dim); L.dE = cv.take<float>(Ba * c.latent_dim); }
     for (int k = 0; k < c.n_disc_units; ++k) L.U[k] = cv.take<float>(Ba * c.disc_units[k]);
     L.Gx = cv.take<float>(Ba * L.amp_ld);
-    int dmax = 0;
-    for (int k = 0; k < c.n_disc_units; ++k) dmax = max(dmax, c.disc_units[k]);
-    gsz = imax64(gsz, 3 * Ba * (int64_t)dmax);
   }
-  L.G0 = cv.take<float>(gsz);
-  L.G1 = cv.take<float>(gsz);
+  L.G0 = cv.take<float>(L.gsz);
+  L.G1 = cv.take<float>(L.gsz);
   L.acc = cv.take<double>(ACC_COUNT);
   for (int k = 0; k < c.n_style_units && L.ase; ++k) L.Sb[k] = cv.take<uint32_t>(Ra * bits_ld(c.style_units[k]));
   for (int k = 0; k < c.n_units; ++k) { L.Hb[k] = cv.take<uint32_t>(Ra * bits_ld(c.units[k])); L.Cb[k] = cv.take<uint32_t>(B * bits_ld(c.units[k])); }
@@ -175,25 +197,13 @@ static void carve(AseLearner& L, void* ws, int64_t* total) {
   L.tc_ws = L.tc_ws_bytes ? cv.take<char>(L.tc_ws_bytes) : nullptr;
   L.reg_dev = (c.gemm_backend == 2) ? cv.take<char>(PlaneRegistry::device_bytes()) : nullptr;
   if (c.gemm_backend >= 1) {
-    // activation planes: registered lazily in register_planes(); size = 2 x (sum of registered fp32 buffers, ld padded to 4)
-    int64_t act = 0;
-    auto add = [&](int64_t rows, int64_t cols) { act += rows * align_up(cols, 4); };
-    add(Ra, L.ldx); if (L.ase) { add(B, L.ldx); add(Ra, c.latent_dim); for (int k = 0; k < c.n_style_units; ++k) add(Ra, c.style_units[k]); }
-    for (int k = 0; k < c.n_units; ++k) { add(Ra, c.units[k]); add(B, c.units[k]); }
-    if (L.amp) {
-      add(3 * Ba, L.amp_ld);
-      for (int k = 0; k < c.n_disc_units; ++k) { add(3 * Ba, c.disc_units[k]); add(Ba, c.disc_units[k]); }
-      add(Ba, L.amp_ld);
-      add(3 * Ba, 1); if (L.ase) add(Ba, c.latent_dim);
-    }
-    add(Ra, c.act_dim); add(B, 1);
-    add(1, gsz); add(1, gsz);
-    L.act_plane_floats = act;
-    L.act_planes = cv.take<float>(2 * act);
-    int64_t wf = 0;
-    for (int i = 0; i < L.net.n_tensors; ++i) wf += (int64_t)L.net.desc[i].rows * align_up(L.net.desc[i].cols, 4);
-    L.w_plane_floats = wf;
-    L.w_planes = cv.take<float>(2 * wf);
+    // one hi/lo plane pair per plane-backed buffer (ld padded to 4), registered lazily in register_planes()
+    int64_t floats[2] = {0, 0};
+    for_each_plane_buf(L, nullptr, [&](const float*, int64_t rows, int64_t cols, bool weight) { floats[weight] += rows * align_up(cols, 4); });
+    L.act_plane_floats = floats[0];
+    L.act_planes = cv.take<float>(2 * floats[0]);
+    L.w_plane_floats = floats[1];
+    L.w_planes = cv.take<float>(2 * floats[1]);
   }
   *total = cv.off;
 }
@@ -201,42 +211,18 @@ static void carve(AseLearner& L, void* ws, int64_t* total) {
 // (Re)build the plane registry: activation buffers once, weight entries whenever the parameter arena pointer changes.
 static void register_planes(AseLearner& L, const float* params) {
   if (L.cfg.gemm_backend < 1) return;
-  const AseLearnerConfig& c = L.cfg;
-  if (!L.reg) { L.reg = new PlaneRegistry; if (c.gemm_backend == 2) { L.reg->f16 = true; L.reg->attach_device(L.reg_dev); } }
+  if (!L.reg) { L.reg = new PlaneRegistry; if (L.cfg.gemm_backend == 2) { L.reg->f16 = true; L.reg->attach_device(L.reg_dev); } }
   if (L.reg->n > 0 && L.reg_params == params) return;
   PlaneRegistry& R = *L.reg;
   R.n = 0;
-  float* hp = L.act_planes; float* lp = L.act_planes + L.act_plane_floats;
-  int64_t off = 0;
-  auto add = [&](const float* base, int64_t rows, int64_t cols) {
+  int64_t off[2] = {0, 0};
+  for_each_plane_buf(L, params, [&](const float* base, int64_t rows, int64_t cols, bool weight) {
+    float* hi = weight ? L.w_planes : L.act_planes;
+    float* lo = hi + (weight ? L.w_plane_floats : L.act_plane_floats);
     const int64_t cap = rows * align_up(cols, 4);
-    R.add(base, rows * cols, hp + off, lp + off, cap);
-    off += cap;
-  };
-  const int64_t Ra = L.Ra, B = L.B, Ba = L.Ba;
-  add(L.Xa, Ra, L.ldx);
-  if (L.ase) { add(L.Xc, B, L.ldx); add(L.Zc, Ra, c.latent_dim); for (int k = 0; k < c.n_style_units; ++k) add(L.S[k], Ra, c.style_units[k]); }
-  for (int k = 0; k < c.n_units; ++k) { add(L.H[k], Ra, c.units[k]); add(L.C[k], B, c.units[k]); }
-  int64_t gsz = Ra * (int64_t)L.maxw;
-  if (L.amp) {
-    add(L.Xd, 3 * Ba, L.amp_ld);
-    int dmax = 0;
-    for (int k = 0; k < c.n_disc_units; ++k) { add(L.D[k], 3 * Ba, c.disc_units[k]); add(L.U[k], Ba, c.disc_units[k]); dmax = max(dmax, c.disc_units[k]); }
-    add(L.Gx, Ba, L.amp_ld);
-    gsz = imax64(gsz, 3 * Ba * (int64_t)dmax);
-  }
-  add(L.G0, 1, gsz); add(L.G1, 1, gsz);
-  // head gradients (written by the loss kernels): split once for their dW and dX consumers
-  add(L.dMU, Ra, c.act_dim); add(L.dV, B, 1);
-  if (L.amp) { add(L.dLOGIT, 3 * Ba, 1); if (L.ase) add(L.dE, Ba, c.latent_dim); }
-  float* wh = L.w_planes; float* wl = L.w_planes + L.w_plane_floats;
-  int64_t woff = 0;
-  for (int i = 0; i < L.net.n_tensors; ++i) {
-    const TensorDesc& d = L.net.desc[i];
-    const int64_t cap = (int64_t)d.rows * align_up(d.cols, 4);
-    if (d.rows > 1 || true) R.add(params + d.off, (int64_t)d.rows * d.cols, wh + woff, wl + woff, cap);
-    woff += cap;
-  }
+    R.add(base, rows * cols, hi + off[weight], lo + off[weight], cap);
+    off[weight] += cap;
+  });
   L.reg_params = params;
   L.weights_split = false;
 }
@@ -270,6 +256,8 @@ static int init_learner(AseLearner& L, const AseLearnerConfig& cfg) {
   for (int k = 0; k < cfg.n_units; ++k) mw = max(mw, cfg.units[k]);
   if (L.ase) { for (int k = 0; k < cfg.n_style_units; ++k) mw = max(mw, cfg.style_units[k]); mw = max(mw, cfg.latent_dim); }
   L.maxw = mw;
+  L.gsz = (int64_t)L.Ra * mw;
+  for (int k = 0; k < cfg.n_disc_units && L.amp; ++k) L.gsz = imax64(L.gsz, 3 * (int64_t)L.Ba * cfg.disc_units[k]);
   return ASE_OK;
 }
 

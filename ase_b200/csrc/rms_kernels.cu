@@ -3,9 +3,9 @@
 // the parallel-Welford rule of the reference, and the normalise/clamp pass uses the UPDATED statistics
 // exactly as the reference's train-mode forward does.  Up to 3 batches can be merged sequentially in one
 // launch (the three AMP batches of calc_gradients, ase_agent.py:170-181).
-#include <cuda_fp16.h>
 #include "common.cuh"
 #include "kernels.h"
+#include "tc_common.cuh"
 
 namespace ase {
 
@@ -80,15 +80,6 @@ rms_finalize_kernel(const double2* __restrict__ partial, int cols, int chunks, i
 
 __global__ void rms_count_add_kernel(double* count, double inc) { count[0] += inc; }
 
-__device__ __forceinline__ void split_tf32_rms(float x, float& hi, float& lo) {   // same split as gemm_tc.cu (operand planes)
-  uint32_t h, l;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(h) : "f"(x));
-  hi = __uint_as_float(h);
-  const float rr = x - hi;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(l) : "f"(rr));
-  lo = __uint_as_float(l);
-}
-
 // y = clamp((x-mean)/std, -5, 5) written to up to 3 destinations (unnorm: std*clamp(x,+-5)+mean).
 // Threads map to columns (coalesced rows, the column's mean / std loaded once), blockIdx.y walks chunks of rows.
 constexpr int NORM_ROWS_PER_BLOCK = 8;       // few rows per thread, all loads in flight at once: the pass is latency-bound otherwise
@@ -114,8 +105,8 @@ rms_normalize_kernel(const float* __restrict__ x, int64_t ldx, int rows, int col
     float h = 0.0f, l = 0.0f;
     __half hh = __float2half_rn(0.0f), hl = hh;
     if (planes) {
-      if (!dst.half) split_tf32_rms(y, h, l);
-      else { const float ys = y * dst.pscale; hh = __float2half_rn(ys); hl = __float2half_rn(ys - __half2float(hh)); }
+      if (!dst.half) split_tf32(y, h, l);
+      else split_f16(y * dst.pscale, hh, hl);
     }
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
@@ -151,16 +142,17 @@ rms_normalize_vec4_kernel(const float* __restrict__ x, int64_t ldx, int rows, in
     const float v[4] = {xv[i].x, xv[i].y, xv[i].z, xv[i].w};
     const float m4[4] = {mu.x, mu.y, mu.z, mu.w}, s4[4] = {sd.x, sd.y, sd.z, sd.w};
     float y[4], h[4], l[4];
-    __half hh[4], hl[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       if (unnorm) y[j] = s4[j] * fminf(fmaxf(v[j], -5.0f), 5.0f) + m4[j];
       else y[j] = fminf(fmaxf((v[j] - m4[j]) / s4[j], -5.0f), 5.0f);
-      h[j] = l[j] = 0.0f; hh[j] = hl[j] = __float2half_rn(0.0f);
-      if (planes) {
-        if (!dst.half) split_tf32_rms(y[j], h[j], l[j]);
-        else { const float ys = y[j] * dst.pscale; hh[j] = __float2half_rn(ys); hl[j] = __float2half_rn(ys - __half2float(hh[j])); }
-      }
+      h[j] = l[j] = 0.0f;
+      if (planes && !dst.half) split_tf32(y[j], h[j], l[j]);
+    }
+    uint2 hv = make_uint2(0u, 0u), lv = hv;
+    if (planes && dst.half) {
+      split_f16x2(y[0] * dst.pscale, y[1] * dst.pscale, hv.x, lv.x);
+      split_f16x2(y[2] * dst.pscale, y[3] * dst.pscale, hv.y, lv.y);
     }
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
@@ -171,10 +163,8 @@ rms_normalize_vec4_kernel(const float* __restrict__ x, int64_t ldx, int rows, in
           *reinterpret_cast<float4*>((float*)dst.hi[d] + o) = make_float4(h[0], h[1], h[2], h[3]);
           *reinterpret_cast<float4*>((float*)dst.lo[d] + o) = make_float4(l[0], l[1], l[2], l[3]);
         } else {
-          const __half2 a = __halves2half2(hh[0], hh[1]), b = __halves2half2(hh[2], hh[3]);
-          const __half2 e = __halves2half2(hl[0], hl[1]), f = __halves2half2(hl[2], hl[3]);
-          *reinterpret_cast<uint2*>((__half*)dst.hi[d] + o) = make_uint2(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b));
-          *reinterpret_cast<uint2*>((__half*)dst.lo[d] + o) = make_uint2(*reinterpret_cast<const uint32_t*>(&e), *reinterpret_cast<const uint32_t*>(&f));
+          *reinterpret_cast<uint2*>((__half*)dst.hi[d] + o) = hv;
+          *reinterpret_cast<uint2*>((__half*)dst.lo[d] + o) = lv;
         }
       }
     }
@@ -186,23 +176,19 @@ __global__ void __launch_bounds__(256)
 copy_cols_kernel(const float* __restrict__ x, int64_t ldx, int rows, int cols, float* __restrict__ y, int64_t ldy,
                  void* __restrict__ hi, void* __restrict__ lo, int64_t ldp, int half, float pscale, unsigned* __restrict__ flag) {
   const int64_t total = (int64_t)rows * cols;
-  bool over = false;
+  float m = 0.0f;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int r = (int)(i / cols), c = (int)(i - (int64_t)r * cols);
     const float v = x[(int64_t)r * ldx + c];
     y[(int64_t)r * ldy + c] = v;
     if (hi) {
       const int64_t o = (int64_t)r * ldp + c;
-      if (!half) { float h, l; split_tf32_rms(v, h, l); ((float*)hi)[o] = h; ((float*)lo)[o] = l; }
-      else {
-        const float vs = v * pscale;
-        over |= fabsf(vs) > 60000.0f;
-        const __half hh = __float2half_rn(vs);
-        ((__half*)hi)[o] = hh; ((__half*)lo)[o] = __float2half_rn(vs - __half2float(hh));
-      }
+      if (!half) { float h, l; split_tf32(v, h, l); ((float*)hi)[o] = h; ((float*)lo)[o] = l; }
+      else { __half h, l; split_f16(v * pscale, h, l); ((__half*)hi)[o] = h; ((__half*)lo)[o] = l; m = fmaxf(m, fabsf(v)); }
     }
   }
-  if (over && flag) atomicOr(flag, 1u);       // the static plane scale assumes bounded inputs (unit latents): report instead of saturating silently
+  // the static plane scale assumes bounded inputs (unit latents): report instead of saturating silently
+  if (hi && half) report_scale_miss(m, pscale, nullptr, flag);
 }
 
 int64_t rms_scratch_bytes(int cols, int rows, int nbatch) {

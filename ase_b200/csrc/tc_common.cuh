@@ -1,5 +1,6 @@
 // Shared device-side pieces of the wgmma GEMM kernel (gemm_tc.cu): PTX wrappers (mbarrier, TMA, wgmma), shared-memory
-// descriptors, the hi/lo split helpers and the epilogue parameter block.
+// descriptors, the hi/lo split helpers with their scale-miss report (also used by the normaliser kernels, rms_kernels.cu, which
+// write operand planes too) and the epilogue parameter block.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -150,6 +151,21 @@ __device__ __forceinline__ float scale_from_amax(float amax, int top) {
   int e; frexpf(amax, &e);                      // amax = m * 2^e, m in [0.5, 1)
   return ldexpf(1.0f, max(-100, min(100, top - e)));
 }
+
+// ------------------------------------------------------------------------------------------ the hi/lo split (every writer of planes)
+__device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
+  uint32_t h, l;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(h) : "f"(x));
+  hi = __uint_as_float(h);
+  const float r = x - hi;                       // exact
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(l) : "f"(r));
+  lo = __uint_as_float(l);
+}
+// FP16 format: xs is the value already multiplied by its scale
+__device__ __forceinline__ void split_f16(float xs, __half& hi, __half& lo) {
+  hi = __float2half_rn(xs);
+  lo = __float2half_rn(xs - __half2float(hi));   // the residual is exact in fp32
+}
 // two elements at once: cvt.rn.f16x2.f32 (F2FP, full rate) instead of two scalar F2F conversions (quarter-rate pipe; ncu r01:
 // the store phase stalled on MIO at the F2Fs); the residuals are exact in fp32.  Returns the packed hi / lo half2 words.
 __device__ __forceinline__ void split_f16x2(float a, float b, uint32_t& hi, uint32_t& lo) {
@@ -159,27 +175,25 @@ __device__ __forceinline__ void split_f16x2(float a, float b, uint32_t& hi, uint
   hi = *reinterpret_cast<const uint32_t*>(&h);
   lo = *reinterpret_cast<const uint32_t*>(&l);
 }
+// FP16 format, end of a pass that wrote planes with scale s: m is the thread's running max |x|.  The warp's max goes into amax_out
+// (the scale source of the next call) and a scale that does not fit the data is reported in the sticky flag: bit 0 when a scaled
+// value exceeds 60000 (never saturate silently), bit 1 when the site only ever saw all-zero tensors and now there is data.  Both
+// pointers may be null.  The warp shuffles: call it from every lane of the warp.
+__device__ __forceinline__ void report_scale_miss(float m, float s, unsigned* amax_out, unsigned* flag) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0 && m > 0.0f) {
+    if (amax_out) atomicMax(amax_out, __float_as_uint(m));        // non-negative floats order like their uint bits
+    if (flag && !(m * s <= 60000.0f)) atomicOr(flag, 1u);
+    if (flag && s == 0.0f) atomicOr(flag, 2u);
+  }
+}
+
 // explicit shared-space accesses for the staging tile (a generic pointer makes the compiler emit LD.E / ST.E with their longer latency)
 __device__ __forceinline__ float4 lds128(const float* p) {
   float4 v;
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(smem_u32(p)));
   return v;
-}
-__device__ __forceinline__ void sts128(float* p, float a, float b, float c, float d) {
-  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(smem_u32(p)), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-__device__ __forceinline__ void split_f16(float xs, __half& hi, __half& lo) {
-  hi = __float2half_rn(xs);
-  lo = __float2half_rn(xs - __half2float(hi));   // the residual is exact in fp32
-}
-
-__device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
-  uint32_t h, l;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(h) : "f"(x));
-  hi = __uint_as_float(h);
-  const float r = x - hi;                       // exact
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(l) : "f"(r));
-  lo = __uint_as_float(l);
 }
 
 struct TcEpi {
@@ -209,13 +223,4 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
-}  // namespace ase
-
-// ------------------------------------------------------------------------------------------ host side (shared between the .cu files)
-namespace ase {
-// per-launch CUDA-event timing of the GEMM kernels (ase_gemm_tc_profile); defined in gemm_tc.cu
-bool tc_prof_on();
-void tc_prof_mark(cudaStream_t st);
-void tc_prof_add_flops(double f);
-int tc_pdl();
 }  // namespace ase

@@ -228,3 +228,45 @@ def test_fp16_plane_scale_window_edges():
     fresh()
     assert _plane_flags(ln) == 0
     print('plane-scale window (f: worst ref32-vs-fp64, worst ours-vs-fp64):', worst)
+
+
+def test_fp16_plane_scale_miss_of_split_writers():
+    """The two writers of FP16 planes that are not GEMM epilogues report a scale miss themselves, and each case below can only be
+    flagged by that writer: a GEMM epilogue downstream would flag the same growth and hide a broken report.
+
+    Latent columns (copy_cols) are written into planes with the static scale 64.  Right after params_changed every scale site
+    calibrates exactly, so only static-scale writers can flag: a latent entry of 1000 (64000 after scaling) must set bit 0, one of
+    900 (57600) must not.
+
+    Weights are re-split in one batched launch with the scale predicted from their last exact split: adam_step marks the weight planes
+    stale but keeps their sites known.  mu.weight grown x 512 without params_changed must set bit 0 in the next eval_actor_critic, x 64
+    must not.  The mu output has no planes, so with want_value=False no epilogue can flag in its place."""
+    _threads()
+    from ase_b200 import Learner
+    c = CASES['ase_ragged']
+    cfg = oracle_cfg(c)
+    P, st, _ = states(c, seed=5)
+    d, new_z = minibatch(c, st, cfg, seed=50)
+    dc, nz = _cuda(d), new_z.cuda()
+    ln = Learner(**learner_kwargs(c, cfg), gemm_backend=2)
+    n = c['B'] - 37
+    obs, z = dc['obs'][:n], dc['ase_latents'][:n]
+
+    for v, flagged in ((900.0, False), (1000.0, True)):
+        ln.load_named(P)                                 # params_changed: every scale site calibrates exactly on the next call
+        x = dict(dc); x['ase_latents'] = dc['ase_latents'].clone()
+        x['ase_latents'][7, 5] = v
+        ln.calc_gradients(x, nz, update_rms=False)
+        assert _plane_flags(ln) == (1 if flagged else 0), v
+        ln.plane_flag_clear()
+
+    for f, flagged in ((64.0, False), (512.0, True)):
+        ln.load_named(P)
+        ln.train_result(ln.calc_gradients(dc, nz, update_rms=False))     # calibration (train_result raises on a flag)
+        ln.eval_actor_critic(obs, z, want_value=False)
+        assert _plane_flags(ln) == 0, f
+        ln.adam_step()
+        ln.named_parameters()['mu.weight'].mul_(f)
+        ln.eval_actor_critic(obs, z, want_value=False)
+        assert _plane_flags(ln) == (1 if flagged else 0), f
+        ln.plane_flag_clear()
