@@ -7,7 +7,7 @@ import importlib
 
 _LAZY = {'lib': '.lib', 'ops': '.ops', 'learner': '.learner', 'agent': '.agent', 'synthetic_env': '.synthetic_env',
          'replay_buffer': '.replay_buffer', 'build': '.build', 'motion_lib': '.motion_lib', 'configs': '.configs',
-         'dist_utils': '.dist_utils'}
+         'dist_utils': '.dist_utils', 'player': '.player'}
 __all__ = ['lib', 'ops', 'Learner', 'param_names', 'build']
 
 

@@ -28,6 +28,38 @@ from .learner import Learner
 from .replay_buffer import ReplayBuffer
 
 
+def net_params(config):
+    """YAML `network` section: from rl_games' model builder when dropped into run.py, else config['net_params']."""
+    net = config.get('network')
+    if net is not None and hasattr(net, 'network_builder'):
+        return net.network_builder.params
+    return config['net_params']
+
+
+def build_frozen_llc(config, env_info, obs_dim, latent_dim, num_envs, device):
+    """The frozen ASE low-level controller of HRLAgent and HRLPlayer (hrl_agent.py:202-213, hrl_players.py:210-221), in eval mode:
+    config['llc_learner'] as it is, or a Learner of config['llc_net_params'] widths holding config['llc_checkpoint'] (an rl_games .pth such as
+    ase/data/models/ase_llc_reallusion_sword_shield.pth); without a checkpoint, the reference initialisation."""
+    ln = config.get('llc_learner')
+    if ln is None:
+        np_ = config['llc_net_params']
+        amp_dim = env_info['amp_observation_space'].shape[0]
+        act = env_info['action_space'].shape[0]
+        ln = Learner('ase', obs_dim, act, num_envs, amp_dim=amp_dim, latent_dim=latent_dim, amp_batch=max(2, num_envs),
+                     units=tuple(np_['mlp']['units']), disc_units=tuple(np_['disc']['units']), device=device,
+                     gemm_backend=config.get('gemm_backend', 2))
+        ckpt = config.get('llc_checkpoint')
+        if ckpt:
+            w = torch.load(ckpt, map_location='cpu', weights_only=True)
+            ln.load_state_dict(w['model'])
+            ln.set_stats_weights(w)
+        else:
+            ln.init_reference(seed=1)
+    for r in (ln.running_mean_std, ln.value_mean_std, ln.amp_input_mean_std):
+        r.eval()
+    return ln
+
+
 def swap_and_flatten01(x):
     """rl_games a2c_common.swap_and_flatten01: env-major flatten, row = env * H + t."""
     s = x.shape
@@ -142,11 +174,7 @@ class CommonAgent:
         pass
 
     def _net_params(self, config):
-        """YAML `network` section: from rl_games' model builder when dropped into run.py, else config['net_params']."""
-        net = config.get('network')
-        if net is not None and hasattr(net, 'network_builder'):
-            return net.network_builder.params
-        return config['net_params']
+        return net_params(config)
 
     def _learner_kwargs(self, config):
         np_ = self._net_params(config)
@@ -978,24 +1006,7 @@ class HRLAgent(CommonAgent):
         self.actions_num = self._latent_dim            # hrl_agent.py:171-174 _setup_action_space
 
     def _build_llc(self, config):
-        ln = config.get('llc_learner')
-        if ln is None:
-            np_ = config['llc_net_params']
-            amp_dim = self.env_info['amp_observation_space'].shape[0]
-            act = self.env_info['action_space'].shape[0]
-            ln = Learner('ase', self.obs_shape[0] - self._task_size, act, self.num_actors, amp_dim=amp_dim, latent_dim=self._latent_dim,
-                         amp_batch=max(2, self.num_actors), units=tuple(np_['mlp']['units']), disc_units=tuple(np_['disc']['units']),
-                         device=self.ppo_device, gemm_backend=config.get('gemm_backend', 2))
-            ckpt = config.get('llc_checkpoint')
-            if ckpt:
-                w = torch.load(ckpt, map_location='cpu', weights_only=True)
-                ln.load_state_dict(w['model'])
-                ln.set_stats_weights(w)
-            else:
-                ln.init_reference(seed=1)
-        for r in (ln.running_mean_std, ln.value_mean_std, ln.amp_input_mean_std):
-            r.eval()
-        self._llc = ln
+        self._llc = build_frozen_llc(config, self.env_info, self.obs_shape[0] - self._task_size, self._latent_dim, self.num_actors, self.ppo_device)
 
     def init_tensors(self):
         super().init_tensors()

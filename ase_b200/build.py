@@ -9,7 +9,7 @@ CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'csrc')
 LIB = os.path.join(CSRC, 'libase_b200.so')
 OBJ = os.path.join(CSRC, 'build')
 SOURCES = ['api.cu', 'obs_kernels.cu', 'rms_kernels.cu', 'rollout_kernels.cu', 'gemm_simt.cu', 'gemm_tc.cu',
-           'loss_kernels.cu', 'learner.cu', 'motion_kernels.cu', 'reset_kernels.cu', 'comm.cu', 'peer.cu']
+           'loss_kernels.cu', 'learner.cu', 'motion_kernels.cu', 'reset_kernels.cu', 'player_kernels.cu', 'comm.cu', 'peer.cu']
 HEADERS = ['common.cuh', 'kernels.h', 'tc_common.cuh', 'philox.cuh', 'motion_common.cuh', os.path.join('..', '..', 'include', 'ase_b200.h')]
 NVCC_FLAGS = ['-O3', '-std=c++17', '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-Xcompiler', '-fPIC']
 

@@ -34,5 +34,23 @@ __device__ __forceinline__ uint4 philox_u4(const uint64_t* rng, uint32_t sid, ui
   const uint64_t seed = rng[0], call = rng[1];
   return philox4x32_10(make_uint4(row, grp, (uint32_t)call, (uint32_t)(call >> 32)), make_uint2((uint32_t)seed, (uint32_t)(seed >> 32) ^ (sid * 0x9E3779B1u)));
 }
+// One warp writes latent row `row` to `out`: normalize(randn(Z)) from stream `sid` (ase_network_builder.py:221-225; F.normalize eps 1e-12),
+// or the injected final row z_in (copied as is).  Z <= 128: lane l owns components 4l .. 4l+3.  Shared by the rollout's and the player's
+// latent kernels, so both draw the same latents from the same counter.
+__device__ __forceinline__ void warp_write_latent(float* __restrict__ out, int Z, const uint64_t* __restrict__ rng, uint32_t sid, uint32_t row,
+                                                  const float* __restrict__ z_in) {
+  const int lane = threadIdx.x & 31;
+  float v[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+  float ss = 0.0f;
+  for (int j0 = lane * 4; j0 < Z; j0 += 128) {
+    if (z_in) { for (int q = 0; q < 4 && j0 + q < Z; ++q) v[q] = z_in[j0 + q]; }
+    else { const float4 t = philox_normal4(rng, sid, row, (uint32_t)(j0 >> 2)); v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w; }
+    for (int q = 0; q < 4 && j0 + q < Z; ++q) ss += v[q] * v[q];
+  }
+  ss = warp_sum(ss);
+  const float inv = 1.0f / fmaxf(sqrtf(ss), 1e-12f);
+  for (int j0 = lane * 4; j0 < Z; j0 += 128)
+    for (int q = 0; q < 4 && j0 + q < Z; ++q) out[j0 + q] = z_in ? v[q] : v[q] * inv;
+}
 
 }  // namespace ase

@@ -257,17 +257,7 @@ latent_update_kernel(float* __restrict__ latents, int Z, int32_t* __restrict__ r
   const int32_t cur = reset_steps[e];
   const bool update = !reset && ((int64_t)cur <= progress[e]);
   if (!reset && !update) return;                   // warp-uniform
-  float v[4] = {0.0f, 0.0f, 0.0f, 0.0f};
-  float ss = 0.0f;
-  for (int j0 = lane * 4; j0 < Z; j0 += 128) {     // Z <= 128: one group of 4 per lane
-    if (z_in) { for (int q = 0; q < 4 && j0 + q < Z; ++q) v[q] = z_in[(int64_t)e * Z + j0 + q]; }
-    else { const float4 t = philox_normal4(rng, (uint32_t)sid, (uint32_t)e, (uint32_t)(j0 >> 2)); v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w; }
-    for (int q = 0; q < 4 && j0 + q < Z; ++q) ss += v[q] * v[q];
-  }
-  ss = warp_sum(ss);
-  const float inv = 1.0f / fmaxf(sqrtf(ss), 1e-12f);
-  for (int j0 = lane * 4; j0 < Z; j0 += 128)
-    for (int q = 0; q < 4 && j0 + q < Z; ++q) latents[(int64_t)e * Z + j0 + q] = z_in ? v[q] : v[q] * inv;
+  warp_write_latent(latents + (int64_t)e * Z, Z, rng, (uint32_t)sid, (uint32_t)e, z_in ? z_in + (int64_t)e * Z : nullptr);
   if (lane == 0) {
     int32_t r;
     if (steps_in) r = steps_in[e];

@@ -110,7 +110,7 @@ class TrainResult(C.Structure):
 
 # every symbol declared in include/ase_b200.h (tests/test_abi.py checks the two lists agree)
 EXPORTS = ['ase_abi_version', 'ase_last_error', 'ase_launch_count', 'ase_obs_build', 'ase_amp_obs_build',
-           'ase_rms_scratch_bytes', 'ase_rms_update', 'ase_rms_apply', 'ase_gae', 'ase_amp_rewards', 'ase_heading_obs', 'ase_heading_reward', 'ase_location_obs', 'ase_location_reward', 'ase_reach_obs', 'ase_reach_reward', 'ase_strike_obs', 'ase_strike_reward', 'ase_motion_state', 'ase_amp_obs_demo', 'ase_policy_sample', 'ase_policy_sample_rng', 'ase_latent_update', 'ase_rollout_post_step', 'ase_humanoid_reset', 'ase_strike_reset', 'ase_task_resample', 'ase_amp_state_init', 'ase_amp_history_init', 'ase_recovery_step', 'ase_adv_normalize', 'ase_gather_rows',
+           'ase_rms_scratch_bytes', 'ase_rms_update', 'ase_rms_apply', 'ase_gae', 'ase_amp_rewards', 'ase_heading_obs', 'ase_heading_reward', 'ase_location_obs', 'ase_location_reward', 'ase_reach_obs', 'ase_reach_reward', 'ase_strike_obs', 'ase_strike_reward', 'ase_motion_state', 'ase_amp_obs_demo', 'ase_policy_sample', 'ase_policy_sample_rng', 'ase_latent_update', 'ase_rollout_post_step', 'ase_player_latents', 'ase_player_act', 'ase_player_scratch_bytes', 'ase_player_post_step', 'ase_humanoid_reset', 'ase_strike_reset', 'ase_task_resample', 'ase_amp_state_init', 'ase_amp_history_init', 'ase_recovery_step', 'ase_adv_normalize', 'ase_gather_rows',
            'ase_gemm', 'ase_gemm_tc_workspace_bytes', 'ase_gemm_tc_plan', 'ase_gemm_tc_profile', 'ase_gemm_tc_profile_read', 'ase_learner_num_params', 'ase_learner_param_desc',
            'ase_learner_arena_floats', 'ase_learner_workspace_bytes', 'ase_learner_create', 'ase_learner_destroy', 'ase_learner_params_changed', 'ase_learner_plane_status', 'ase_learner_plane_flag_to', 'ase_learner_plane_flag_clear',
            'ase_learner_calc_gradients', 'ase_learner_adam_step', 'ase_learner_eval_actor_critic',
@@ -153,6 +153,10 @@ def _load():
     lib.ase_policy_sample_rng.argtypes = [vp, vp, vp, i32, i32, vp, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.ase_latent_update.argtypes = [vp, i32, vp, vp, vp, i32, i32, i32, vp, i32, vp, vp, vp]
     lib.ase_rollout_post_step.argtypes = [vp, vp, vp, vp, vp, vp, f32, i32, vp, vp, vp, vp, vp, vp]
+    lib.ase_player_latents.argtypes = [vp, i32, vp, i32, i32, vp, i32, vp, vp]
+    lib.ase_player_act.argtypes = [vp, vp, i32, i32, vp, vp, vp, i32, vp, vp, vp, vp]
+    lib.ase_player_scratch_bytes.argtypes = [i32]
+    lib.ase_player_post_step.argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, i64, vp, vp, vp, vp, vp]
     lib.ase_humanoid_reset.argtypes = [vp, vp, i64, i64, vp, i64, i64, i32, vp, vp, f32, i32, i32, vp, vp, vp]
     lib.ase_strike_reset.argtypes = [vp, vp, i64, i64, vp, i64, i64, i32, vp, vp, vp, vp, i64, f32, i32, i32, vp, vp, vp]
     lib.ase_task_resample.argtypes = [C.POINTER(TaskParams), vp, i64, vp, vp, i32, vp, i64, vp, vp, vp, vp, i32, vp, vp, vp]

@@ -137,6 +137,36 @@ def rollout_post_step(rewards, dones, terminate, v_next_normed, value_rms, next_
                                     _p(meter), _p(rng), _stream()), 'ase_rollout_post_step')
 
 
+def player_latents(latents, done_mask, resample_all, rng, stream_id, z_in=None):
+    """ASEPlayer._reset_latents(done ids) (done_mask) or of every env (resample_all), mask driven (ase_players.py:61-94)."""
+    n, z = latents.shape
+    assert latents.is_contiguous() and (done_mask is None or done_mask.dtype == torch.uint8)
+    check(lib.ase_player_latents(_p(latents), z, _p(done_mask), int(bool(resample_all)), n, _p(rng), int(stream_id), _p(z_in), _stream()),
+          'ase_player_latents')
+
+
+def player_act(mu, logstd, low, high, rng, stream_id, actions=None, unit_out=None, noise=None):
+    """A player's action from the head output mu: Normal.sample when logstd is given (else mu), clamp to [-1, 1], rescale_actions(low, high)
+    into `actions` and / or the L2-normalised clamped action into `unit_out` (ase_players.py:54-59, hrl_players.py:53-60,243-249)."""
+    rows, a = mu.shape
+    mu = _f32c(mu, 'mu')
+    check(lib.ase_player_act(_p(mu), _p(logstd), rows, a, _p(low), _p(high), _p(rng), int(stream_id), _p(noise), _p(actions), _p(unit_out),
+                             _stream()), 'ase_player_act')
+
+
+def player_post_step(rewards, dones, sub_step, llc_steps, sub_rewards, sub_dones, cr, steps, done_out, n_games, status, record, scratch, rng):
+    """CommonPlayer.run's bookkeeping after env.step (common_player.py:73-117; HRL sub-steps hrl_players.py:174-191) into the device
+    AsePlayerStatus `status` (a uint8 tensor of its 32 bytes) and this step's record (3 float64)."""
+    n = cr.shape[0]
+    rewards = _f32c(rewards.reshape(n), 'rewards')
+    dones = dones.reshape(n)
+    if dones.dtype != torch.uint8:
+        dones = dones.to(torch.uint8)
+    check(lib.ase_player_post_step(_p(rewards), _p(dones.contiguous()), n, int(sub_step), int(llc_steps), _p(sub_rewards), _p(sub_dones), _p(cr),
+                                   _p(steps), _p(done_out), int(n_games), _p(status), _p(record), _p(scratch), _p(rng), _stream()),
+          'ase_player_post_step')
+
+
 def compute_humanoid_reset(progress_buf, contact_buf, is_contact_body, body_state, max_episode_length, enable_early_termination,
                            termination_heights, reset_out=None, terminate_out=None):
     """env/tasks/humanoid.py:645-670 -> (reset, terminated) uint8 [N].  contact_buf [N, J, 3]; body_state [N, J, 13];

@@ -199,6 +199,37 @@ int ase_latent_update(float* latents, int latent_dim, int32_t* reset_steps, cons
 int ase_rollout_post_step(const float* rewards, const uint8_t* dones, const uint8_t* terminate, const float* v_next_normed,
                           const double* val_mean, const double* val_var, float eps, int num_envs, float* next_values,
                           float* cur_rewards, float* cur_lengths, float* meter, uint64_t* rng, void* stream);
+/* ---- evaluation players (learning/common_player.py, amp_players.py, ase_players.py, hrl_players.py) ----------------------------------------
+ * CommonPlayer.run reads `done.nonzero()` and two .item() sums back every step.  These entry points keep the step mask driven: the episode
+ * statistics accumulate on the device in an AsePlayerStatus, and the host reads it once per window of steps.  Draws follow the addressing
+ * above (rng / stream_id); the caller's ase_player_post_step advances rng[1] once per player step. */
+typedef struct {
+  double reward_sum;        /* run totals over the counted episodes: fp64 sums of their accumulated reward and step count */
+  double steps_sum;
+  int64_t games_played;     /* episodes counted so far */
+  int32_t stopped;          /* sticky: set by the step that took games_played to >= n_games; later launches change nothing */
+  uint32_t ticket;          /* block ticket of the running launch; 0 between launches */
+} AsePlayerStatus;
+/* ase_players.py:61-94: every env flagged in done_mask (_reset_latents(done_ids)), or every env when resample_all (_update_latents), gets
+ * latent = normalize(randn(Z)) (the same device function as ase_latent_update).  z_in [N, Z] (final latents) replaces the draws. */
+int ase_player_latents(float* latents, int latent_dim, const uint8_t* done_mask, int resample_all, int num_envs, const uint64_t* rng,
+                       int stream_id, const float* z_in, void* stream);
+/* ase_players.py:54-59, hrl_players.py:53-60,243-249: a = mu, or mu + exp(logstd) * eps when logstd is non-NULL (stochastic; eps from the
+ * Philox stream or noise_in [rows, A]); a := clamp(a, -1, 1).  actions (optional) = rescale_actions(low, high, a) with per-component bounds
+ * (a itself when low/high are NULL); unit_out (optional) = normalize(a), the HRL high-level step's latent for the LLC.  act_dim <= 128. */
+int ase_player_act(const float* mu, const float* logstd, int rows, int act_dim, const float* low, const float* high, const uint64_t* rng,
+                   int stream_id, const float* noise_in, float* actions, float* unit_out, void* stream);
+/* bytes of the per-block partial sums ase_player_post_step needs for num_envs envs */
+int ase_player_scratch_bytes(int num_envs);
+/* CommonPlayer.run after env.step (common_player.py:73-117).  Sub-step mode (llc_steps > 1, HRLPlayer.env_step hrl_players.py:174-191):
+ * sub_rewards / sub_dones accumulate r and d over sub_step = 0 .. llc_steps - 1; the last sub-step forms r = sum / llc_steps, d = count > 0
+ * and runs the rest.  Per env: cr += r, steps += 1, done_out = d; for the done envs, record[0..2] = {count, sum of cr, sum of steps} (fp64,
+ * reduced per block and then in block order by the last block to finish), added to the status totals, and their cr / steps zeroed.  A step
+ * that takes games_played to >= n_games counts in full and sets status->stopped.  While stopped is set the launch changes nothing (record
+ * included), so the caller zeroes the records it hands in.  Called with llc_steps == 1 and sub_step 0 outside HRL. */
+int ase_player_post_step(const float* rewards, const uint8_t* dones, int num_envs, int sub_step, int llc_steps, float* sub_rewards,
+                         float* sub_dones, float* cr, float* steps, uint8_t* done_out, int64_t n_games, AsePlayerStatus* status,
+                         double* record, void* scratch, uint64_t* rng, void* stream);
 /* compute_humanoid_reset, env/tasks/humanoid.py:645-670: contact forces [N, J, 3] (strides in floats), rigid-body state as in ase_obs_build,
  * is_contact_body [J] flags the bodies allowed to touch the ground (contact_body_ids), termination_heights [J]. */
 int ase_humanoid_reset(const int64_t* progress, const float* contact, int64_t contact_env_stride, int64_t contact_body_stride,
