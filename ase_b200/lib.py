@@ -111,7 +111,10 @@ class TrainResult(C.Structure):
 # every symbol declared in include/ase_b200.h (tests/test_abi.py checks the two lists agree)
 EXPORTS = ['ase_abi_version', 'ase_last_error', 'ase_launch_count', 'ase_obs_build', 'ase_amp_obs_build',
            'ase_rms_scratch_bytes', 'ase_rms_update', 'ase_rms_apply', 'ase_gae', 'ase_amp_rewards', 'ase_heading_obs', 'ase_heading_reward', 'ase_location_obs', 'ase_location_reward', 'ase_reach_obs', 'ase_reach_reward', 'ase_strike_obs', 'ase_strike_reward', 'ase_motion_state', 'ase_amp_obs_demo', 'ase_policy_sample', 'ase_policy_sample_rng', 'ase_latent_update', 'ase_rollout_post_step', 'ase_player_latents', 'ase_player_act', 'ase_player_scratch_bytes', 'ase_player_post_step', 'ase_humanoid_reset', 'ase_strike_reset', 'ase_task_resample', 'ase_amp_state_init', 'ase_amp_history_init', 'ase_recovery_step', 'ase_adv_normalize', 'ase_gather_rows',
-           'ase_gemm', 'ase_gemm_tc_workspace_bytes', 'ase_gemm_tc_plan', 'ase_gemm_tc_profile', 'ase_gemm_tc_profile_read', 'ase_learner_num_params', 'ase_learner_param_desc',
+           'ase_gemm', 'ase_gemm_tc_workspace_bytes', 'ase_gemm_tc_plan', 'ase_gemm_tc_profile', 'ase_gemm_tc_profile_read',
+           'ase_gemm_planes_device_bytes', 'ase_gemm_planes_create', 'ase_gemm_planes_destroy', 'ase_gemm_planes_add', 'ase_gemm_planes_begin_call',
+           'ase_gemm_planes_forget', 'ase_gemm_planes_prep_weights', 'ase_gemm_planes_gemm', 'ase_gemm_planes_info', 'ase_gemm_planes_status',
+           'ase_gemm_planes_clear', 'ase_learner_num_params', 'ase_learner_param_desc',
            'ase_learner_arena_floats', 'ase_learner_workspace_bytes', 'ase_learner_create', 'ase_learner_destroy', 'ase_learner_params_changed', 'ase_learner_plane_status', 'ase_learner_plane_flag_to', 'ase_learner_plane_flag_clear',
            'ase_learner_calc_gradients', 'ase_learner_adam_step', 'ase_learner_eval_actor_critic',
            'ase_learner_eval_disc_enc', 'ase_comm_load', 'ase_comm_unique_id', 'ase_comm_create', 'ase_comm_destroy', 'ase_grad_allreduce',
@@ -173,6 +176,17 @@ def _load():
     lib.ase_gemm_tc_plan.argtypes = [i32, i32, i32, i32, i32, i32, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.ase_gemm_tc_profile.argtypes = [i32]
     lib.ase_gemm_tc_profile_read.argtypes = [C.POINTER(C.c_double), C.POINTER(i64), C.POINTER(C.c_double)]
+    lib.ase_gemm_planes_device_bytes.argtypes = []; lib.ase_gemm_planes_device_bytes.restype = i64
+    lib.ase_gemm_planes_create.argtypes = [i32, vp, C.POINTER(vp)]
+    lib.ase_gemm_planes_destroy.argtypes = [vp]; lib.ase_gemm_planes_destroy.restype = None
+    lib.ase_gemm_planes_add.argtypes = [vp, vp, i64, vp, vp, i64]
+    lib.ase_gemm_planes_begin_call.argtypes = [vp, i32, vp]
+    lib.ase_gemm_planes_forget.argtypes = [vp]
+    lib.ase_gemm_planes_prep_weights.argtypes = [vp, C.POINTER(vp), C.POINTER(i32), C.POINTER(i32), i32, vp]
+    lib.ase_gemm_planes_gemm.argtypes = [vp, C.POINTER(GemmParams), vp]
+    lib.ase_gemm_planes_info.argtypes = [vp, vp, C.POINTER(i64), vp, vp]
+    lib.ase_gemm_planes_status.argtypes = [vp, C.POINTER(i32), vp]
+    lib.ase_gemm_planes_clear.argtypes = [vp, vp]
     lib.ase_learner_num_params.argtypes = [C.POINTER(LearnerConfig)]
     lib.ase_learner_param_desc.argtypes = [C.POINTER(LearnerConfig), i32, C.POINTER(i64), C.POINTER(i32), C.POINTER(i32)]
     lib.ase_learner_arena_floats.argtypes = [C.POINTER(LearnerConfig)]

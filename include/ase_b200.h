@@ -385,6 +385,30 @@ int ase_gemm_tc_plan(int M, int N, int K, int accumulate, int split_k, int backe
  * summed kernel time, the launch count and the algorithmic FLOPs (2*M*N*Kpad per launch). */
 int ase_gemm_tc_profile(int enable);
 int ase_gemm_tc_profile_read(double* total_ms, int64_t* launches, double* flops);
+/* The operand-plane registry the learner runs its tensor-core GEMMs through, exposed (for tests) behind an opaque handle: fp32
+ * buffers registered with hi/lo planes in caller memory (TF32 words for backend 1, scaled FP16 halfs for backend 2, stored in the
+ * same float space), per-call scale sites, weights split in one batched pass.  Each function maps onto one registry operation:
+ *   create      backend 1 or 2; device_mem: >= ase_gemm_planes_device_bytes() (backend 2 only, zero-filled here; may be NULL for 1)
+ *   add         register an fp32 buffer of capacity_floats and its planes (plane_capacity_floats floats each)
+ *   begin_call  start of one stream-ordered sequence of GEMMs whose scale sites start at site_base (backend 2: re-predicts scales)
+ *   forget      the parameters changed: every scale is re-derived exactly on the next call
+ *   prep_weights  split each srcs[i] (contiguous [rows[i], cols[i]], registered) at weight site i, count <= 40
+ *   gemm        ase_gemm through the registry (p->backend must match)
+ *   info        out[6] = valid, fp32_stale, rows, cols, ld, ldp of the buffer registered at `base`; if the planes are valid (backend 2)
+ *               and scale_dst is set, [scale, 1/scale] they were written with is copied to scale_dst (device, stream-ordered)
+ *   status      the sticky scale-miss flag of backend 2 (bits as ase_learner_plane_status), one stream synchronisation; clear resets it */
+typedef struct AseGemmPlanes AseGemmPlanes;
+int64_t ase_gemm_planes_device_bytes(void);
+int ase_gemm_planes_create(int backend, void* device_mem, AseGemmPlanes** out);
+void ase_gemm_planes_destroy(AseGemmPlanes* h);
+int ase_gemm_planes_add(AseGemmPlanes* h, const float* base, int64_t capacity_floats, float* hi, float* lo, int64_t plane_capacity_floats);
+int ase_gemm_planes_begin_call(AseGemmPlanes* h, int site_base, void* stream);
+int ase_gemm_planes_forget(AseGemmPlanes* h);
+int ase_gemm_planes_prep_weights(AseGemmPlanes* h, const float* const* srcs, const int* rows, const int* cols, int count, void* stream);
+int ase_gemm_planes_gemm(AseGemmPlanes* h, const AseGemmParams* p, void* stream);
+int ase_gemm_planes_info(AseGemmPlanes* h, const float* base, int64_t* out, float* scale_dst, void* stream);
+int ase_gemm_planes_status(AseGemmPlanes* h, int* flags, void* stream);
+int ase_gemm_planes_clear(AseGemmPlanes* h, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Learner: one PPO + adversarial minibatch update.  Replaces
