@@ -12,8 +12,10 @@
 // producer into a shared-memory ring with mbarrier completion; warpgroups 1, 2 = BM / 2 rows each: wgmma into register
 // fragments, every (k-block, m64 block)'s partial -- corrections and A_hi.B_hi -- added into fp32 registers with
 // round-to-nearest adds -- the tensor core's own accumulation truncates.
-// Store phase: registers -> shared staging tile -> coalesced pass with bias / ReLU / tanh / mask (fp32 or 1-bit), optional
-// fp32 C, half planes (predicted power-of-two scale), ReLU activity bits, max |C|, fused column sums, split-K fp32 RED.
+// Store phase: bias / ReLU / tanh / mask (fp32 or 1-bit), optional fp32 C, half planes (predicted power-of-two scale), ReLU
+// activity bits, max |C|, fused column sums, split-K fp32 RED.  Interior, aligned 128-column tiles are stored straight from
+// the accumulator fragments (epilogue_frag: no staging tile, no CTA-wide barrier, one quad shuffle per value pair so that a
+// lane stores 4 consecutive columns); every other tile goes registers -> shared staging tile -> coalesced pass (epilogue_rows).
 // Descriptor formats follow the PTX ISA "Matrix Descriptor Format" for wgmma.  DESIGN.md section 5 has the numerics.
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -122,12 +124,9 @@ __device__ __forceinline__ void epilogue_rows(const TcEpi& e, const float* cs, i
   if ((e.c_amax || (H && e.Chi && e.flag)) && !e.accumulate) report_scale_miss(amax, cscale, e.c_amax, (H && e.Chi) ? e.flag : nullptr);
 }
 
-// Fast store phase for interior, aligned tiles of BN = 128 (the generic epilogue_rows above handles everything else).
-// The generic loop spends ~500 issue slots per (row, 4-column) item on predicates, 64-bit address arithmetic and scalar tails
-// (ncu r01b: 43 % of the kernel's lifetime, issue-bound, not memory-bound).  Here a lane owns 8 consecutive columns of each of the
-// warp's 16 rows: two LDS.128 from the staged tile, one 16-byte store per half plane, pointers advanced by the row strides, the
-// rows' activity-mask words prefetched before the loop, no bounds checks.
-__device__ __forceinline__ bool epilogue_fast_ok(const TcEpi& e, int m0, int n0, int bm, int bn, bool H) {
+// Interior, aligned tiles of BN = 128 without split-K accumulation take the fragment store phase (epilogue_frag below); the
+// staged, generic epilogue_rows above handles everything else.
+__device__ __forceinline__ bool epilogue_frag_ok(const TcEpi& e, int m0, int n0, int bm, int bn, bool H) {
   if (e.accumulate || m0 + bm > e.M || n0 + bn > e.N) return false;
   if ((e.ldc & 3) || (reinterpret_cast<uintptr_t>(e.C) & 15)) return false;
   if (e.bias && (reinterpret_cast<uintptr_t>(e.bias) & 15)) return false;
@@ -136,121 +135,146 @@ __device__ __forceinline__ bool epilogue_fast_ok(const TcEpi& e, int m0, int n0,
   return true;
 }
 
-// CPL = columns per lane (8: 256-wide tile, 4: 128-wide tile), NR = rows per warp (a multiple of 4)
-template <bool H, int CPL, int NR>
-__device__ __forceinline__ void epilogue_fast(const TcEpi& e, const float* cs, int cs_ld, float* s_colsum, int row0, int m0, int n0, int lane) {
-  static_assert(CPL == 4 || CPL == 8, "columns per lane");
-  constexpr int LPW = 32 / CPL;                        // lanes per 32-column activity word
-  const int c8 = lane * CPL, n = n0 + c8;
-  const int64_t m = m0 + row0;
-  float bv[CPL];
-#pragma unroll
-  for (int j = 0; j < CPL; ++j) bv[j] = 0.0f;
-  if (e.bias) {
-#pragma unroll
-    for (int j = 0; j < CPL; j += 4) {
-      const float4 b0 = *reinterpret_cast<const float4*>(e.bias + n + j);
-      bv[j] = b0.x; bv[j + 1] = b0.y; bv[j + 2] = b0.z; bv[j + 3] = b0.w;
-    }
-  }
+// Fragment store phase: every consumer thread applies the epilogue to the accumulators it holds and stores them itself -- no
+// staging tile, no CTA-wide barrier, so a warpgroup starts storing while the other one still computes, and the operand ring is
+// never touched.  m64n128 fragment layout: thread t of a warpgroup holds rows 16 (t/32) + (t%32)/4 and + 8 of each m64 block and
+// the column pairs 8 j + 2 (t%4), j = 0..15.  Per 16-column group (two j) the lanes of a quad swap one pair with their
+// neighbour (shfl.xor 1): even lanes then own columns 2 q .. 2 q + 3 of the group, odd lanes 8 + 2 (q - 1) .. + 3, so a lane
+// stores one float4 of C and one uint2 per half plane, and a quad writes whole 32-byte sectors.  A lane's four columns are
+// one nibble of the row's 32-column activity word: two groups are OR-ed over the quad into the whole word, and lane q stores
+// the word of the thread's q-th row; mask words are read whole by every lane.  Column sums: the thread's rows first, then the
+// warp's 8 row lanes (shfl.xor 4 / 8 / 16), then shared-memory atomics into s_colsum.
+// Every element sees the operations of epilogue_rows in the same order, so C, the planes and the activity bits are
+// bit-identical to it; the multiplies and the bias add are spelled __fmul_rn / __fadd_rn because here -- with no shared-memory
+// round trip between them -- the compiler would contract them into an FMA.
+// The per-thread arrays of epilogue_frag.  A struct, not a bare array: the compiler merges the stack slots of equally typed bare
+// arrays of the functions it inlines into the kernel, epilogue_rows indexes its float[4] / uint32_t[2] arrays dynamically, and a
+// merged slot keeps every store of epilogue_frag's (register-resident) arrays alive as local-memory traffic.
+template <class T, int N> struct FragArr {
+  T v[N];
+  __device__ __forceinline__ T& operator[](int i) { return v[i]; }
+  __device__ __forceinline__ const T& operator[](int i) const { return v[i]; }
+};
+
+template <bool H, int NH>
+__device__ __forceinline__ void epilogue_frag(const TcEpi& e, float (&acc)[NH][64], float* s_colsum, int m0, int n0, int wg, int t) {
+  constexpr int NROW = 2 * NH;                               // rows per thread; row k is 64 (k / 2) + 8 (k % 2) below the first
+  constexpr unsigned FULL = 0xffffffffu;
+  const int lane = t & 31, q = lane & 3;
+  const bool odd = q & 1;
+  const int cq = ((q & 1) << 3) | ((q & 2) << 1);            // this lane's 4 columns inside a 16-column group: 0, 8, 4, 12
+  const int64_t m = m0 + wg * NH * 64 + 16 * (t >> 5) + (lane >> 2);
+  const int n = n0 + cq;
+  // FP16 planes: undo the operands' power-of-two scales (two exact multiplies; their product alone could underflow)
+  const float s1 = (H && e.a_inv) ? *e.a_inv : 1.0f;
+  const float s2 = e.alpha * ((H && e.b_inv) ? *e.b_inv : 1.0f);
   const float cscale = (H && e.Chi && e.c_scale) ? *e.c_scale : 1.0f;
   const bool use_bits = e.mask_mode == 1 && e.mask_bits != nullptr;
-  const int sh = CPL * (lane & (LPW - 1));             // this lane's bits of the 32-column activity word
-  // activity-mask words: 4 rows per group, the next group's words are in flight while the current one is processed
-  const uint32_t* mb = use_bits ? e.mask_bits + m * e.ldmb + (n >> 5) : nullptr;
-  uint32_t mw[4] = {0, 0, 0, 0}, mwn[4] = {0, 0, 0, 0};
+  const uint32_t* mb = use_bits ? e.mask_bits + m * e.ldmb + (n0 >> 5) : nullptr;
+  float* cp = e.C + m * e.ldc + n;
+  __half* hp = (H && e.Chi) ? (__half*)e.Chi + m * e.ldp + n : nullptr;
+  __half* lp = (H && e.Chi) ? (__half*)e.Clo + m * e.ldp + n : nullptr;
+  const float* mp = (e.mask_mode && !use_bits) ? e.mask_src + m * e.ldm + n : nullptr;
+  const float* bp = e.bias ? e.bias + n : nullptr;
+  FragArr<uint32_t, NROW> mw, mwn;                             // the rows' mask words: the next 32 columns' are in flight
+#pragma unroll
+  for (int k = 0; k < NROW; ++k) { mw[k] = 0; mwn[k] = 0; }
   if (use_bits) {
 #pragma unroll
-    for (int r = 0; r < 4; ++r) mw[r] = __ldg(mb + (int64_t)r * e.ldmb);
+    for (int k = 0; k < NROW; ++k) mw[k] = __ldg(mb + (64 * (k >> 1) + 8 * (k & 1)) * e.ldmb);
   }
-  float* cp = e.C + m * e.ldc + n;
-  __half* hp = e.Chi ? (__half*)e.Chi + m * e.ldp + n : nullptr;
-  __half* lp = e.Chi ? (__half*)e.Clo + m * e.ldp + n : nullptr;
-  uint32_t* rb = e.relu_bits ? e.relu_bits + m * e.ldrb + (n >> 5) : nullptr;
-  const float* mp = (e.mask_mode && !use_bits) ? e.mask_src + m * e.ldm + n : nullptr;
-  const float* sp = cs + row0 * cs_ld + c8;
-  float csum[CPL];
-#pragma unroll
-  for (int j = 0; j < CPL; ++j) csum[j] = 0.0f;
   float amax = 0.0f;
+  FragArr<uint32_t, NROW> rbw;                              // the rows' activity words: two groups each
+#pragma unroll
+  for (int k = 0; k < NROW; ++k) rbw[k] = 0;
+  // One 16-column group (fragment column blocks j = 2 g, 2 g + 1) per trip of a ROLLED loop: the group is always read from
+  // the first 8 registers of each m64 block and the rest move down by 8 at the end of the trip (56 MOVs per block).  Unrolled
+  // over the 8 groups the store phase is ~120 KB of straight-line code that every warp walks once per tile, and it ran at
+  // the speed of the instruction fetch: twice as long as the staged store phase it replaces.
 #pragma unroll 1
-  for (int g = 0; g < NR / 4; ++g) {
-    if (use_bits && g + 1 < NR / 4) {
+  for (int g = 0; g < 8; ++g) {
+    const int w = g >> 1;                                    // 32 columns: one word of activity / mask bits per row
+    if (use_bits && !(g & 1) && w < 3) {
 #pragma unroll
-      for (int r = 0; r < 4; ++r) mwn[r] = __ldg(mb + (int64_t)(4 * (g + 1) + r) * e.ldmb);
+      for (int k = 0; k < NROW; ++k) mwn[k] = __ldg(mb + (64 * (k >> 1) + 8 * (k & 1)) * e.ldmb + w + 1);
     }
+    const int c = 16 * g, sh = 16 * (g & 1) + cq;          // sh: this lane's nibble of the word
+    FragArr<float, 4> bv = {{0.0f, 0.0f, 0.0f, 0.0f}};
+    if (bp) { const float4 b4 = *reinterpret_cast<const float4*>(bp + c); bv[0] = b4.x; bv[1] = b4.y; bv[2] = b4.z; bv[3] = b4.w; }
+    FragArr<float, 4> csum = {{0.0f, 0.0f, 0.0f, 0.0f}};
 #pragma unroll
-    for (int r = 0; r < 4; ++r) {
-      float x[CPL];
+    for (int k = 0; k < NROW; ++k) {
+      const int64_t ro = 64 * (k >> 1) + 8 * (k & 1);
+      const float* a = acc[k >> 1] + 2 * (k & 1);          // a[0..1]: block 2 g, a[4..5]: block 2 g + 1
+      const float r0 = __shfl_xor_sync(FULL, odd ? a[0] : a[4], 1), r1 = __shfl_xor_sync(FULL, odd ? a[1] : a[5], 1);
+      FragArr<float, 4> x;
+      x[0] = odd ? r0 : a[0]; x[1] = odd ? r1 : a[1]; x[2] = odd ? a[4] : r0; x[3] = odd ? a[5] : r1;
 #pragma unroll
-      for (int j = 0; j < CPL; j += 4) {
-        const float4 t = lds128(sp + j);
-        x[j] = t.x + bv[j]; x[j + 1] = t.y + bv[j + 1]; x[j + 2] = t.z + bv[j + 2]; x[j + 3] = t.w + bv[j + 3];
-      }
+      for (int j = 0; j < 4; ++j) x[j] = __fadd_rn(__fmul_rn(s2, __fmul_rn(s1, x[j])), bv[j]);
       if (e.act == 1) {
 #pragma unroll
-        for (int j = 0; j < CPL; ++j) x[j] = fmaxf(x[j], 0.0f);
+        for (int j = 0; j < 4; ++j) x[j] = fmaxf(x[j], 0.0f);
       } else if (e.act == 2) {
 #pragma unroll
-        for (int j = 0; j < CPL; ++j) x[j] = tanhf(x[j]);
+        for (int j = 0; j < 4; ++j) x[j] = tanhf(x[j]);
       }
-      if (rb) {              // a lane's bits are one byte (CPL = 8) / one nibble (CPL = 4) of the row's little-endian activity words
-        uint32_t w = 0;
+      if (e.relu_bits) {
+        uint32_t nib = 0;
 #pragma unroll
-        for (int j = 0; j < CPL; ++j) w |= (x[j] > 0.0f) ? (1u << j) : 0u;
-        if (CPL == 8) reinterpret_cast<uint8_t*>(rb)[lane & 3] = (uint8_t)w;
-        else {
-          w |= __shfl_xor_sync(0xffffffffu, w << 4, 1) & 0xF0u;          // even lanes pick up the odd neighbour's nibble
-          if (!(lane & 1)) reinterpret_cast<uint8_t*>(rb)[(lane & 7) >> 1] = (uint8_t)w;
-        }
-        rb += e.ldrb;
+        for (int j = 0; j < 4; ++j) nib |= (x[j] > 0.0f) ? (1u << j) : 0u;
+        rbw[k] |= nib << sh;
       }
       if (use_bits) {
 #pragma unroll
-        for (int j = 0; j < CPL; ++j) x[j] = ((mw[r] >> (sh + j)) & 1u) ? x[j] : 0.0f;
+        for (int j = 0; j < 4; ++j) x[j] = ((mw[k] >> (sh + j)) & 1u) ? x[j] : 0.0f;
       } else if (mp) {
-        float mv[CPL];
-#pragma unroll
-        for (int j = 0; j < CPL; j += 4) {
-          const float4 q = *reinterpret_cast<const float4*>(mp + j);
-          mv[j] = q.x; mv[j + 1] = q.y; mv[j + 2] = q.z; mv[j + 3] = q.w;
-        }
+        const float4 q4 = *reinterpret_cast<const float4*>(mp + ro * e.ldm + c);
+        const FragArr<float, 4> mv = {{q4.x, q4.y, q4.z, q4.w}};
         if (e.mask_mode == 1) {
 #pragma unroll
-          for (int j = 0; j < CPL; ++j) x[j] = (mv[j] > 0.0f) ? x[j] : 0.0f;
+          for (int j = 0; j < 4; ++j) x[j] = (mv[j] > 0.0f) ? x[j] : 0.0f;
         } else {
 #pragma unroll
-          for (int j = 0; j < CPL; ++j) x[j] *= (1.0f - mv[j] * mv[j]);
+          for (int j = 0; j < 4; ++j) x[j] *= (1.0f - mv[j] * mv[j]);
         }
-        mp += e.ldm;
       }
-      if (!e.skip_c) {
+      if (!e.skip_c) *reinterpret_cast<float4*>(cp + ro * e.ldc + c) = make_float4(x[0], x[1], x[2], x[3]);
 #pragma unroll
-        for (int j = 0; j < CPL; j += 4) *reinterpret_cast<float4*>(cp + j) = make_float4(x[j], x[j + 1], x[j + 2], x[j + 3]);
-      }
-#pragma unroll
-      for (int j = 0; j < CPL; ++j) { csum[j] += x[j]; amax = fmaxf(amax, fabsf(x[j])); }
+      for (int j = 0; j < 4; ++j) { csum[j] += x[j]; amax = fmaxf(amax, fabsf(x[j])); }
       if (H && hp) {
-        uint32_t hw[CPL / 2], lw[CPL / 2];
-#pragma unroll
-        for (int j = 0; j < CPL; j += 2) split_f16x2(x[j] * cscale, x[j + 1] * cscale, hw[j >> 1], lw[j >> 1]);
-        if (CPL == 8) {
-          *reinterpret_cast<uint4*>(hp) = make_uint4(hw[0], hw[1], hw[CPL / 2 - 2], hw[CPL / 2 - 1]);
-          *reinterpret_cast<uint4*>(lp) = make_uint4(lw[0], lw[1], lw[CPL / 2 - 2], lw[CPL / 2 - 1]);
-        } else {
-          *reinterpret_cast<uint2*>(hp) = make_uint2(hw[0], hw[1]);
-          *reinterpret_cast<uint2*>(lp) = make_uint2(lw[0], lw[1]);
-        }
-        hp += e.ldp; lp += e.ldp;
+        uint2 hv, lv;
+        split_f16x2(x[0] * cscale, x[1] * cscale, hv.x, lv.x); split_f16x2(x[2] * cscale, x[3] * cscale, hv.y, lv.y);
+        *reinterpret_cast<uint2*>(hp + ro * e.ldp + c) = hv;
+        *reinterpret_cast<uint2*>(lp + ro * e.ldp + c) = lv;
       }
-      cp += e.ldc; sp += cs_ld;
+    }
+    if (e.colsum) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        float v = csum[j];
+        v += __shfl_xor_sync(FULL, v, 4); v += __shfl_xor_sync(FULL, v, 8); v += __shfl_xor_sync(FULL, v, 16);
+        if (lane < 4) atomicAdd(s_colsum + c + cq + j, v);
+      }
+    }
+    if (e.relu_bits && (g & 1)) {
+      uint32_t word = 0;
+#pragma unroll
+      for (int k = 0; k < NROW; ++k) {
+        uint32_t v = rbw[k];
+        v |= __shfl_xor_sync(FULL, v, 1); v |= __shfl_xor_sync(FULL, v, 2);
+        if (q == k) word = v;
+        rbw[k] = 0;
+      }
+      if (q < NROW) e.relu_bits[(m + 64 * (q >> 1) + 8 * (q & 1)) * e.ldrb + (n0 >> 5) + w] = word;
+    }
+    if (g & 1) {
+#pragma unroll
+      for (int k = 0; k < NROW; ++k) mw[k] = mwn[k];
     }
 #pragma unroll
-    for (int r = 0; r < 4; ++r) mw[r] = mwn[r];
-  }
-  if (e.colsum) {
+    for (int h = 0; h < NH; ++h)
 #pragma unroll
-    for (int j = 0; j < CPL; ++j) atomicAdd(s_colsum + c8 + j, csum[j]);
+      for (int i = 0; i < 56; ++i) acc[h][i] = acc[h][i + 8];
   }
   if (e.c_amax || (H && e.Chi && e.flag)) report_scale_miss(amax, cscale, e.c_amax, (H && e.Chi) ? e.flag : nullptr);
 }
@@ -263,8 +287,9 @@ struct TcSmem {
   static constexpr int A_BYTES = BM * 128;                   // per plane: one 128-byte k-block row per operand row
   static constexpr int B_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
-  static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-  static_assert(BM * (BN + 4) * 4 + BN * 4 <= STAGES * STAGE_BYTES, "the store phase's staging tile lives over the ring");
+  static constexpr int COLSUM_OFF = STAGES * STAGE_BYTES + 256;   // [BN] fp32 column sums, behind the barriers: never over the ring
+  static constexpr int TOTAL = COLSUM_OFF + 512 + 1024 /*align slack*/;
+  static_assert(BM * (BN + 4) * 4 <= STAGES * STAGE_BYTES, "the generic store phase's staging tile lives over the ring");
 };
 
 // one 64 x BN MMA over k-slice k (32 bytes of K) of a k-block; sd = 0 starts a fresh accumulator
@@ -318,6 +343,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant_
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }   // 2 consumer warpgroups release a stage
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
+  float* s_colsum = reinterpret_cast<float*>(smem + SM::COLSUM_OFF);   // per-tile column sums
+  if (threadIdx.x < BN) s_colsum[threadIdx.x] = 0.0f;
   __syncthreads();
   pdl_sync();
 
@@ -390,36 +417,36 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant_
       for (int j = 0; j < R; ++j) acc[h][j] += part[j];    // round-to-nearest fp32 accumulation across k-blocks
     }
   }
-  // Phase 1: accumulators -> shared staging tile [BM][BN+4] over the idle ring (every TMA load was consumed; the barrier
-  // waits for the other warpgroup's last MMAs).  Fragment layout of m64nN: thread t holds rows 16 (t/32) + (t%32)/4 (+8)
-  // and column pairs 8 j + 2 (t%4).
-  asm volatile("bar.sync 1, 256;" ::: "memory");      // the 8 consumer warps only
-  float* cs = reinterpret_cast<float*>(smem);
-  constexpr int CS_LD = BN + 4;
-  // FP16 planes: undo the operands' power-of-two scales (two exact multiplies; their product alone could underflow)
-  const float s1 = (H && e.a_inv) ? *e.a_inv : 1.0f;
-  const float s2 = e.alpha * ((H && e.b_inv) ? *e.b_inv : 1.0f);
-#pragma unroll
-  for (int h = 0; h < NH; ++h) {
-    const int row = (wg * NH + h) * 64 + 16 * (t >> 5) + ((t & 31) >> 2);
-    float* c0 = cs + row * CS_LD + 2 * (t & 3);
-#pragma unroll
-    for (int j = 0; j < R / 4; ++j) {
-      const float* a = acc[h] + 4 * j;
-      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(smem_u32(c0 + 8 * j)), "f"(s2 * (s1 * a[0])), "f"(s2 * (s1 * a[1])) : "memory");
-      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(smem_u32(c0 + 8 * CS_LD + 8 * j)), "f"(s2 * (s1 * a[2])), "f"(s2 * (s1 * a[3])) : "memory");
-    }
-  }
-  float* s_colsum = cs + BM * CS_LD;                  // [BN] per-tile column sums, behind the staging tile
   const int et = threadIdx.x - 128;                   // 0..255 within the consumer warps
-  if (e.colsum && et < BN) s_colsum[et] = 0.0f;
-  asm volatile("bar.sync 1, 256;" ::: "memory");
-  // Phase 2: coalesced epilogue -- consumer warp w owns rows [w BM/8, (w + 1) BM/8)
-  constexpr int NRW = BM / 8;
-  const int ew = warp - 4;
-  if (!(e.debug & 1)) {
-    if (BN == 128 && epilogue_fast_ok(e, m0, n0, BM, BN, H) && !(e.debug & 256)) epilogue_fast<H, 4, NRW>(e, cs, CS_LD, s_colsum, ew * NRW, m0, n0, lane);
-    else epilogue_rows<H>(e, cs, CS_LD, s_colsum, ew * NRW, NRW, BN, m0, n0, lane);
+  bool frag = false;
+  if constexpr (BN == 128) frag = epilogue_frag_ok(e, m0, n0, BM, BN, H) && !(e.debug & 256);
+  if (frag) {
+    if constexpr (BN == 128) { if (!(e.debug & 1)) epilogue_frag<H, NH>(e, acc, s_colsum, m0, n0, wg, t); }
+  } else {
+    // Generic store phase.  Phase 1: accumulators -> shared staging tile [BM][BN+4] over the idle ring (every TMA load was
+    // consumed; the barrier waits for the other warpgroup's last MMAs).  Fragment layout of m64nN: thread t holds rows
+    // 16 (t/32) + (t%32)/4 (+8) and column pairs 8 j + 2 (t%4).
+    asm volatile("bar.sync 1, 256;" ::: "memory");      // the 8 consumer warps only
+    float* cs = reinterpret_cast<float*>(smem);
+    constexpr int CS_LD = BN + 4;
+    // FP16 planes: undo the operands' power-of-two scales (two exact multiplies; their product alone could underflow)
+    const float s1 = (H && e.a_inv) ? *e.a_inv : 1.0f;
+    const float s2 = e.alpha * ((H && e.b_inv) ? *e.b_inv : 1.0f);
+#pragma unroll
+    for (int h = 0; h < NH; ++h) {
+      const int row = (wg * NH + h) * 64 + 16 * (t >> 5) + ((t & 31) >> 2);
+      float* c0 = cs + row * CS_LD + 2 * (t & 3);
+#pragma unroll
+      for (int j = 0; j < R / 4; ++j) {
+        const float* a = acc[h] + 4 * j;
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(smem_u32(c0 + 8 * j)), "f"(s2 * (s1 * a[0])), "f"(s2 * (s1 * a[1])) : "memory");
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(smem_u32(c0 + 8 * CS_LD + 8 * j)), "f"(s2 * (s1 * a[2])), "f"(s2 * (s1 * a[3])) : "memory");
+      }
+    }
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    // Phase 2: coalesced epilogue -- consumer warp w owns rows [w BM/8, (w + 1) BM/8)
+    constexpr int NRW = BM / 8;
+    if (!(e.debug & 1)) epilogue_rows<H>(e, cs, CS_LD, s_colsum, (warp - 4) * NRW, NRW, BN, m0, n0, lane);
   }
   if (e.colsum && !e.accumulate) {
     asm volatile("bar.sync 1, 256;" ::: "memory");

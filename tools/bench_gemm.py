@@ -4,7 +4,10 @@
                                                        Ba = 4096): per shape the tile plan, kernel time, algorithmic TFLOP/s,
                                                        operand bytes the CTAs load and their rate, and the same shape with
                                                        the tile height pinned to 128 rows (ASE_TC_DEBUG bit 512, in a
-                                                       subprocess: the library reads the bits once per process)"""
+                                                       subprocess: the library reads the bits once per process)
+  python tools/bench_gemm.py [backend] --minibatch --store-share
+                                                       the second column is the same shape with the store phase dropped
+                                                       (ASE_TC_DEBUG bit 1) instead: what the store phase costs per shape"""
 import ctypes as C
 import json
 import os
@@ -120,14 +123,15 @@ if '--minibatch' in sys.argv:
     if '--json' in sys.argv:
         print(json.dumps(rows))
         sys.exit(0)
-    env = dict(os.environ, ASE_TC_DEBUG=str(int(os.environ.get('ASE_TC_DEBUG', '0')) | 512))
+    other_bit, other = (1, 'no store') if '--store-share' in sys.argv else (512, 'pinned 128')
+    env = dict(os.environ, ASE_TC_DEBUG=str(int(os.environ.get('ASE_TC_DEBUG', '0')) | other_bit))
     r = subprocess.run([sys.executable, os.path.abspath(__file__), str(backend), '--minibatch', '--json'], env=env, capture_output=True, text=True)
     pinned = json.loads(r.stdout.strip().splitlines()[-1]) if r.returncode == 0 else None
     if pinned is None:
         sys.stderr.write(r.stderr)
     print(f"# backend {backend}, {torch.cuda.get_device_name()}; operand bytes = hi/lo plane bytes all CTAs load per launch")
     print(f"{'gemm':16s} {'M':>6s} {'N':>5s} {'K':>6s}  {'plan':>11s} {'us':>8s} {'TFLOP/s':>8s} {'GB':>6s} {'TB/s':>5s}  |"
-          f" {'pinned 128':>11s} {'us':>8s} {'TFLOP/s':>8s} {'GB':>6s} {'TB/s':>5s}")
+          f" {other:>11s} {'us':>8s} {'TFLOP/s':>8s} {'GB':>6s} {'TB/s':>5s}")
     tot = [0.0, 0.0, 0.0, 0.0]
     for i, a in enumerate(rows):
         fmt = lambda x: (f"{x['plan'][0]}x{x['plan'][1]}/{x['plan'][2]}" if x['plan'] else '-') + \
@@ -141,7 +145,7 @@ if '--minibatch' in sys.argv:
         print(line)
     fl = sum(2.0 * a['M'] * a['N'] * a['K'] for a in rows)
     print(f"# minibatch: {tot[0]/1e3:.3f} ms, {fl/tot[0]/1e6:.1f} TFLOP/s, {tot[1]/1e9:.2f} GB operands, {sum(a['ctas'] for a in rows)} CTAs"
-          + (f"  | pinned 128: {tot[2]/1e3:.3f} ms, {fl/tot[2]/1e6:.1f} TFLOP/s, {tot[3]/1e9:.2f} GB operands, "
+          + (f"  | {other}: {tot[2]/1e3:.3f} ms, {fl/tot[2]/1e6:.1f} TFLOP/s, {tot[3]/1e9:.2f} GB operands, "
              f"{sum(b['ctas'] for b in pinned)} CTAs" if pinned else ''))
     sys.exit(0)
 
