@@ -125,8 +125,9 @@ __device__ __forceinline__ void epilogue_rows(const TcEpi& e, const float* cs, i
 }
 
 // Interior, aligned tiles of BN = 128 without split-K accumulation take the fragment store phase (epilogue_frag below); the
-// staged, generic epilogue_rows above handles everything else.
-__device__ __forceinline__ bool epilogue_frag_ok(const TcEpi& e, int m0, int n0, int bm, int bn, bool H) {
+// staged, generic epilogue_rows above handles everything else.  The host asks the same question for a whole launch (tile 0 of a
+// launch whose M and N are whole tiles) to decide whether it may run the persistent kernel.
+__host__ __device__ __forceinline__ bool epilogue_frag_ok(const TcEpi& e, int m0, int n0, int bm, int bn, bool H) {
   if (e.accumulate || m0 + bm > e.M || n0 + bn > e.N) return false;
   if ((e.ldc & 3) || (reinterpret_cast<uintptr_t>(e.C) & 15)) return false;
   if (e.bias && (reinterpret_cast<uintptr_t>(e.bias) & 15)) return false;
@@ -287,8 +288,9 @@ struct TcSmem {
   static constexpr int A_BYTES = BM * 128;                   // per plane: one 128-byte k-block row per operand row
   static constexpr int B_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
-  static constexpr int COLSUM_OFF = STAGES * STAGE_BYTES + 256;   // [BN] fp32 column sums, behind the barriers: never over the ring
-  static constexpr int TOTAL = COLSUM_OFF + 512 + 1024 /*align slack*/;
+  // [2][BN] fp32 column sums, behind the barriers: never over the ring.  The persistent kernel alternates the two slots by tile
+  static constexpr int COLSUM_OFF = STAGES * STAGE_BYTES + 256;
+  static constexpr int TOTAL = COLSUM_OFF + 2 * 512 + 1024 /*align slack*/;
   static_assert(BM * (BN + 4) * 4 <= STAGES * STAGE_BYTES, "the generic store phase's staging tile lives over the ring");
 };
 
@@ -315,12 +317,19 @@ __device__ __forceinline__ void wg_mma(float (&d)[BN / 2], uint32_t a, uint32_t 
 // with mbarrier completion; warpgroups 1 and 2 (232 registers) each own BM / 2 rows of the BM x BN tile as BM / 128 m64
 // blocks -- at BM = 256 two 64 x BN accumulators plus one partial, 192 registers at BN = 128 -- issue their wgmma, and run
 // the store phase.  While one warpgroup waits for its partial and adds it, the other's MMAs keep the tensor core busy.
-template <int BM, int BN, int STAGES, bool AMN, bool BMN, bool H>
+//
+// PERSIST = false: one tile per CTA, blockIdx = (n tile, m tile, K split).  PERSIST = true (launches whose every tile takes the
+// fragment store phase, see gemm_tc): min(tiles, SMs) CTAs, CTA b computes the linear tiles b, b + gridDim.x, ... in the same
+// raster order (n fastest, then m).  Barrier set-up, tensor-map prefetch and the PDL wait happen once per CTA, the ring's
+// stage index and phase parity run on over all of the CTA's k-blocks, and the producer issues the next tile's k-blocks as soon
+// as stages free up -- the fragment store phase never touches the ring, so the next tile's first stages land under it.
+template <int BM, int BN, int STAGES, bool AMN, bool BMN, bool H, bool PERSIST>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant__ CUtensorMap tmAlo,
                const __grid_constant__ CUtensorMap tmBhi, const __grid_constant__ CUtensorMap tmBlo, const TcEpi e) {
   static_assert(H || (!AMN && !BMN), "TF32 wgmma reads K-major operands only");
   static_assert(BM == 128 || BM == 256, "tile height");
+  static_assert(!PERSIST || (H && BN == 128), "the persistent kernel stores every tile from the fragments");
   using SM = TcSmem<BM, BN, STAGES>;
   using F = TcFmt<H>;
   constexpr int R = BN / 2;                        // fragment registers per thread (64 x BN fp32 over 128 threads)
@@ -331,9 +340,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant_
   uint64_t* empty = full + STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
-  const int kb_begin = blockIdx.z * e.kb_per_split;
-  const int nkb = min(e.kb_per_split, e.kb_total - kb_begin);
+  const int kb_begin = PERSIST ? 0 : blockIdx.z * e.kb_per_split;
+  const int nkb = PERSIST ? e.kb_total : min(e.kb_per_split, e.kb_total - kb_begin);
+  const int tiles_n = PERSIST ? e.N / BN : 1;      // persistent launches have whole tiles in M and N
+  const int ntiles = PERSIST ? (e.M / BM) * tiles_n : 1;
+  const int tile0 = PERSIST ? (int)blockIdx.x : 0, tile_step = PERSIST ? (int)gridDim.x : 1;
+  auto tile_m0 = [&](int tile) { return PERSIST ? (tile / tiles_n) * BM : (int)blockIdx.y * BM; };
+  auto tile_n0 = [&](int tile) { return PERSIST ? (tile % tiles_n) * BN : (int)blockIdx.x * BN; };
 
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmAhi)) : "memory");
@@ -343,39 +356,43 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant_
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }   // 2 consumer warpgroups release a stage
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  float* s_colsum = reinterpret_cast<float*>(smem + SM::COLSUM_OFF);   // per-tile column sums
-  if (threadIdx.x < BN) s_colsum[threadIdx.x] = 0.0f;
+  float* s_colsum = reinterpret_cast<float*>(smem + SM::COLSUM_OFF);   // per-tile column sums, [2][BN]
+  if (threadIdx.x < 2 * BN) s_colsum[threadIdx.x] = 0.0f;
   __syncthreads();
   pdl_sync();
 
   if (warp < 4) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (warp == 0 && lane == 0) {
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int s = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        mbar_wait(&empty[s], ph ^ 1);
-        mbar_expect_tx(&full[s], SM::STAGE_BYTES);
-        uint8_t* st = smem + s * SM::STAGE_BYTES;
-        const int k0 = (kb_begin + kb) * F::BK;
-        if (!AMN) {          // K-major planes [rows, K]: one box of BM rows x one k-block
-          tma_load_2d(st, &tmAhi, &full[s], k0, m0);
-          tma_load_2d(st + SM::A_BYTES, &tmAlo, &full[s], k0, m0);
-        } else {             // MN-major planes [K, rows]: boxes of BK k-rows x 128 bytes of m
+      int it = 0;                                  // k-blocks issued over all tiles: ring stage and phase
+      for (int tile = tile0; tile < ntiles; tile += tile_step) {
+        const int m0 = tile_m0(tile), n0 = tile_n0(tile);
+        for (int kb = 0; kb < nkb; ++kb, ++it) {
+          const int s = it % STAGES;
+          const uint32_t ph = (it / STAGES) & 1;
+          mbar_wait(&empty[s], ph ^ 1);
+          mbar_expect_tx(&full[s], SM::STAGE_BYTES);
+          uint8_t* st = smem + s * SM::STAGE_BYTES;
+          const int k0 = (kb_begin + kb) * F::BK;
+          if (!AMN) {          // K-major planes [rows, K]: one box of BM rows x one k-block
+            tma_load_2d(st, &tmAhi, &full[s], k0, m0);
+            tma_load_2d(st + SM::A_BYTES, &tmAlo, &full[s], k0, m0);
+          } else {             // MN-major planes [K, rows]: boxes of BK k-rows x 128 bytes of m
 #pragma unroll
-          for (int b = 0; b < BM / F::MN_BOX; ++b) {
-            tma_load_2d(st + b * F::MN_BOX_BYTES, &tmAhi, &full[s], m0 + b * F::MN_BOX, k0);
-            tma_load_2d(st + SM::A_BYTES + b * F::MN_BOX_BYTES, &tmAlo, &full[s], m0 + b * F::MN_BOX, k0);
+            for (int b = 0; b < BM / F::MN_BOX; ++b) {
+              tma_load_2d(st + b * F::MN_BOX_BYTES, &tmAhi, &full[s], m0 + b * F::MN_BOX, k0);
+              tma_load_2d(st + SM::A_BYTES + b * F::MN_BOX_BYTES, &tmAlo, &full[s], m0 + b * F::MN_BOX, k0);
+            }
           }
-        }
-        if (!BMN) {
-          tma_load_2d(st + 2 * SM::A_BYTES, &tmBhi, &full[s], k0, n0);
-          tma_load_2d(st + 2 * SM::A_BYTES + SM::B_BYTES, &tmBlo, &full[s], k0, n0);
-        } else {
+          if (!BMN) {
+            tma_load_2d(st + 2 * SM::A_BYTES, &tmBhi, &full[s], k0, n0);
+            tma_load_2d(st + 2 * SM::A_BYTES + SM::B_BYTES, &tmBlo, &full[s], k0, n0);
+          } else {
 #pragma unroll
-          for (int b = 0; b < BN / F::MN_BOX; ++b) {
-            tma_load_2d(st + 2 * SM::A_BYTES + b * F::MN_BOX_BYTES, &tmBhi, &full[s], n0 + b * F::MN_BOX, k0);
-            tma_load_2d(st + 2 * SM::A_BYTES + SM::B_BYTES + b * F::MN_BOX_BYTES, &tmBlo, &full[s], n0 + b * F::MN_BOX, k0);
+            for (int b = 0; b < BN / F::MN_BOX; ++b) {
+              tma_load_2d(st + 2 * SM::A_BYTES + b * F::MN_BOX_BYTES, &tmBhi, &full[s], n0 + b * F::MN_BOX, k0);
+              tma_load_2d(st + 2 * SM::A_BYTES + SM::B_BYTES + b * F::MN_BOX_BYTES, &tmBlo, &full[s], n0 + b * F::MN_BOX, k0);
+            }
           }
         }
       }
@@ -385,72 +402,88 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmAhi, const __grid_constant_
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
   const int wg = (warp >> 2) - 1;                  // consumer warpgroup: tile rows [wg BM/2, (wg + 1) BM/2)
   const int t = threadIdx.x & 127;
+  const int et = threadIdx.x - 128;                // 0..255 within the consumer warps
   const bool corrections = !(e.debug & 4);
-  float acc[NH][R], part[R];
+#pragma unroll 1
+  for (int tile = tile0; tile < ntiles; tile += tile_step) {
+    const int ti = tile / tile_step;                 // tiles this CTA has done (tile0 < tile_step)
+    float acc[NH][R], part[R];
 #pragma unroll
-  for (int h = 0; h < NH; ++h)
+    for (int h = 0; h < NH; ++h)
 #pragma unroll
-    for (int j = 0; j < R; ++j) acc[h][j] = 0.0f;
-  for (int kb = 0; kb < nkb; ++kb) {
-    const int s = kb % STAGES;
-    mbar_wait(&full[s], (kb / STAGES) & 1);
-    const uint32_t sa = smem_u32(smem + s * SM::STAGE_BYTES);
-    const uint32_t b_hi = sa + 2 * SM::A_BYTES, b_lo = b_hi + SM::B_BYTES;
+      for (int j = 0; j < R; ++j) acc[h][j] = 0.0f;
+    // The first MMA of a k-block starts a fresh partial under a run-time predicate, so the compiler takes the partial as read
+    // there: without this, the last tile's partial would stay live across the store phase (64 registers: spills at BM = 256)
+    if constexpr (PERSIST) {
 #pragma unroll
-    for (int h = 0; h < NH; ++h) {
-      // m64 block wg NH + h starts (wg NH + h) x 8 KB into each A plane in both layouts
-      const uint32_t a_hi = sa + (wg * NH + h) * TC_M64_BYTES, a_lo = a_hi + SM::A_BYTES;
-      wg_fence();
-      if (corrections) {
+      for (int j = 0; j < R; ++j) part[j] = 0.0f;
+    }
+    for (int kb = 0; kb < nkb; ++kb) {
+      const int it = ti * nkb + kb;                  // k-blocks consumed over all tiles: ring stage and phase
+      const int s = it % STAGES;
+      mbar_wait(&full[s], (it / STAGES) & 1);
+      const uint32_t sa = smem_u32(smem + s * SM::STAGE_BYTES);
+      const uint32_t b_hi = sa + 2 * SM::A_BYTES, b_lo = b_hi + SM::B_BYTES;
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          wg_mma<BN, AMN, BMN, H>(part, a_lo, b_hi, k, k > 0 ? 1 : 0);
-          wg_mma<BN, AMN, BMN, H>(part, a_hi, b_lo, k, 1);
+      for (int h = 0; h < NH; ++h) {
+        // m64 block wg NH + h starts (wg NH + h) x 8 KB into each A plane in both layouts
+        const uint32_t a_hi = sa + (wg * NH + h) * TC_M64_BYTES, a_lo = a_hi + SM::A_BYTES;
+        wg_fence();
+        if (corrections) {
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            wg_mma<BN, AMN, BMN, H>(part, a_lo, b_hi, k, k > 0 ? 1 : 0);
+            wg_mma<BN, AMN, BMN, H>(part, a_hi, b_lo, k, 1);
+          }
+        }
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wg_mma<BN, AMN, BMN, H>(part, a_hi, b_hi, k, (corrections || k > 0) ? 1 : 0);
+        wg_commit();
+        wg_wait<0>();
+        if (h == NH - 1 && t == 0) mbar_arrive(&empty[s]);   // every MMA reading this stage is done
+#pragma unroll
+        for (int j = 0; j < R; ++j) acc[h][j] += part[j];    // round-to-nearest fp32 accumulation across k-blocks
+      }
+    }
+    const int m0 = tile_m0(tile), n0 = tile_n0(tile);
+    // Column sums: the persistent kernel alternates the two slots by tile.  Tile i + 2 reaches slot i & 1 only after every
+    // consumer thread passed the barrier below for tile i + 1, i.e. after it flushed and zeroed its column of tile i.
+    float* cs_slot = s_colsum + (PERSIST ? (ti & 1) * BN : 0);
+    bool frag = PERSIST;
+    if constexpr (BN == 128 && !PERSIST) frag = epilogue_frag_ok(e, m0, n0, BM, BN, H) && !(e.debug & 256);
+    if (frag) {
+      if constexpr (BN == 128) { if (!(e.debug & 1)) epilogue_frag<H, NH>(e, acc, cs_slot, m0, n0, wg, t); }
+    } else if constexpr (!PERSIST) {
+      // Generic store phase.  Phase 1: accumulators -> shared staging tile [BM][BN+4] over the idle ring (every TMA load was
+      // consumed; the barrier waits for the other warpgroup's last MMAs).  Fragment layout of m64nN: thread t holds rows
+      // 16 (t/32) + (t%32)/4 (+8) and column pairs 8 j + 2 (t%4).
+      asm volatile("bar.sync 1, 256;" ::: "memory");      // the 8 consumer warps only
+      float* cs = reinterpret_cast<float*>(smem);
+      constexpr int CS_LD = BN + 4;
+      // FP16 planes: undo the operands' power-of-two scales (two exact multiplies; their product alone could underflow)
+      const float s1 = (H && e.a_inv) ? *e.a_inv : 1.0f;
+      const float s2 = e.alpha * ((H && e.b_inv) ? *e.b_inv : 1.0f);
+#pragma unroll
+      for (int h = 0; h < NH; ++h) {
+        const int row = (wg * NH + h) * 64 + 16 * (t >> 5) + ((t & 31) >> 2);
+        float* c0 = cs + row * CS_LD + 2 * (t & 3);
+#pragma unroll
+        for (int j = 0; j < R / 4; ++j) {
+          const float* a = acc[h] + 4 * j;
+          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(smem_u32(c0 + 8 * j)), "f"(s2 * (s1 * a[0])), "f"(s2 * (s1 * a[1])) : "memory");
+          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(smem_u32(c0 + 8 * CS_LD + 8 * j)), "f"(s2 * (s1 * a[2])), "f"(s2 * (s1 * a[3])) : "memory");
         }
       }
-#pragma unroll
-      for (int k = 0; k < 4; ++k) wg_mma<BN, AMN, BMN, H>(part, a_hi, b_hi, k, (corrections || k > 0) ? 1 : 0);
-      wg_commit();
-      wg_wait<0>();
-      if (h == NH - 1 && t == 0) mbar_arrive(&empty[s]);   // every MMA reading this stage is done
-#pragma unroll
-      for (int j = 0; j < R; ++j) acc[h][j] += part[j];    // round-to-nearest fp32 accumulation across k-blocks
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      // Phase 2: coalesced epilogue -- consumer warp w owns rows [w BM/8, (w + 1) BM/8)
+      constexpr int NRW = BM / 8;
+      if (!(e.debug & 1)) epilogue_rows<H>(e, cs, CS_LD, s_colsum, (warp - 4) * NRW, NRW, BN, m0, n0, lane);
     }
-  }
-  const int et = threadIdx.x - 128;                   // 0..255 within the consumer warps
-  bool frag = false;
-  if constexpr (BN == 128) frag = epilogue_frag_ok(e, m0, n0, BM, BN, H) && !(e.debug & 256);
-  if (frag) {
-    if constexpr (BN == 128) { if (!(e.debug & 1)) epilogue_frag<H, NH>(e, acc, s_colsum, m0, n0, wg, t); }
-  } else {
-    // Generic store phase.  Phase 1: accumulators -> shared staging tile [BM][BN+4] over the idle ring (every TMA load was
-    // consumed; the barrier waits for the other warpgroup's last MMAs).  Fragment layout of m64nN: thread t holds rows
-    // 16 (t/32) + (t%32)/4 (+8) and column pairs 8 j + 2 (t%4).
-    asm volatile("bar.sync 1, 256;" ::: "memory");      // the 8 consumer warps only
-    float* cs = reinterpret_cast<float*>(smem);
-    constexpr int CS_LD = BN + 4;
-    // FP16 planes: undo the operands' power-of-two scales (two exact multiplies; their product alone could underflow)
-    const float s1 = (H && e.a_inv) ? *e.a_inv : 1.0f;
-    const float s2 = e.alpha * ((H && e.b_inv) ? *e.b_inv : 1.0f);
-#pragma unroll
-    for (int h = 0; h < NH; ++h) {
-      const int row = (wg * NH + h) * 64 + 16 * (t >> 5) + ((t & 31) >> 2);
-      float* c0 = cs + row * CS_LD + 2 * (t & 3);
-#pragma unroll
-      for (int j = 0; j < R / 4; ++j) {
-        const float* a = acc[h] + 4 * j;
-        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(smem_u32(c0 + 8 * j)), "f"(s2 * (s1 * a[0])), "f"(s2 * (s1 * a[1])) : "memory");
-        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(smem_u32(c0 + 8 * CS_LD + 8 * j)), "f"(s2 * (s1 * a[2])), "f"(s2 * (s1 * a[3])) : "memory");
-      }
+    if (e.colsum && !e.accumulate) {
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      if (et < BN && n0 + et < e.N) atomicAdd(e.colsum + n0 + et, cs_slot[et]);
+      if (PERSIST && et < BN) cs_slot[et] = 0.0f;
     }
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    // Phase 2: coalesced epilogue -- consumer warp w owns rows [w BM/8, (w + 1) BM/8)
-    constexpr int NRW = BM / 8;
-    if (!(e.debug & 1)) epilogue_rows<H>(e, cs, CS_LD, s_colsum, (warp - 4) * NRW, NRW, BN, m0, n0, lane);
-  }
-  if (e.colsum && !e.accumulate) {
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    if (et < BN && n0 + et < e.N) atomicAdd(e.colsum + n0 + et, s_colsum[et]);
   }
 }
 
@@ -707,17 +740,17 @@ static int tc_pdl() {   // env ASE_TC_PDL=0 launches the GEMMs fully stream-seri
   return v;
 }
 
-template <int BM, int BN, bool AMN, bool BMN, bool H>
+template <int BM, int BN, bool AMN, bool BMN, bool H, bool PERSIST>
 static int launch_tc(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl, const TcEpi& e,
                      int splits, cudaStream_t st) {
   constexpr int STAGES = tc_stages<BM, BN>();
   using SM = TcSmem<BM, BN, STAGES>;
   static bool attr_set = false;
   if (!attr_set) {
-    ASE_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BM, BN, STAGES, AMN, BMN, H>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::TOTAL));
+    ASE_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BM, BN, STAGES, AMN, BMN, H, PERSIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::TOTAL));
     attr_set = true;
   }
-  dim3 grid(ceil_div(e.N, BN), ceil_div(e.M, BM), splits);
+  const dim3 grid = PERSIST ? dim3(min((e.M / BM) * (e.N / BN), NUM_SMS)) : dim3(ceil_div(e.N, BN), ceil_div(e.M, BM), splits);
   const bool prof = g_prof.on;
   if (prof) prof_mark(st);
   cudaLaunchConfig_t cfg = {};
@@ -726,23 +759,23 @@ static int launch_tc(const CUtensorMap& ah, const CUtensorMap& al, const CUtenso
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = tc_pdl();
   cfg.attrs = attr; cfg.numAttrs = 1;
-  ASE_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BM, BN, STAGES, AMN, BMN, H>, ah, al, bh, bl, e));
+  ASE_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BM, BN, STAGES, AMN, BMN, H, PERSIST>, ah, al, bh, bl, e));
   if (prof) { prof_mark(st); g_prof.flops += 2.0 * (double)e.M * (double)e.N * (double)e.K; }
   ASE_LAUNCH_OK();
   return ASE_OK;
 }
 
-template <int BM, int BN, bool H>
+template <int BM, int BN, bool H, bool PERSIST = false>
 static int launch_tc_major(bool amn, bool bmn, const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
                            const TcEpi& e, int splits, cudaStream_t st) {
   if constexpr (!H) {
     if (amn || bmn) { set_error("wgmma GEMM: TF32 operand planes must be K-major"); return ASE_ERR_INVALID; }
-    return launch_tc<BM, BN, false, false, false>(ah, al, bh, bl, e, splits, st);
+    return launch_tc<BM, BN, false, false, false, false>(ah, al, bh, bl, e, splits, st);
   } else {
-    if (!amn && !bmn) return launch_tc<BM, BN, false, false, true>(ah, al, bh, bl, e, splits, st);
-    if (!amn && bmn) return launch_tc<BM, BN, false, true, true>(ah, al, bh, bl, e, splits, st);
-    if (amn && !bmn) return launch_tc<BM, BN, true, false, true>(ah, al, bh, bl, e, splits, st);
-    return launch_tc<BM, BN, true, true, true>(ah, al, bh, bl, e, splits, st);
+    if (!amn && !bmn) return launch_tc<BM, BN, false, false, true, PERSIST>(ah, al, bh, bl, e, splits, st);
+    if (!amn && bmn) return launch_tc<BM, BN, false, true, true, PERSIST>(ah, al, bh, bl, e, splits, st);
+    if (amn && !bmn) return launch_tc<BM, BN, true, false, true, PERSIST>(ah, al, bh, bl, e, splits, st);
+    return launch_tc<BM, BN, true, true, true, PERSIST>(ah, al, bh, bl, e, splits, st);
   }
 }
 
@@ -1049,6 +1082,12 @@ int gemm_tc(const AseGemmParams& p, cudaStream_t st, PlaneRegistry* reg) {
   e.kb_per_split = ceil_div(e.kb_total, plan.splits);
   const int splits = ceil_div(e.kb_total, e.kb_per_split);
   const bool amn = H && p.a_trans, bmn = H && p.b_trans;
+  // Launches whose every tile takes the fragment store phase (whole tiles in M and N, aligned operands, FP16 planes, BN = 128,
+  // no accumulation) run the persistent kernel: the same tiles and arithmetic, one CTA per SM looping over them
+  const bool persist = H && BN == 128 && !(e.debug & (256 | 1024)) && p.M % plan.bm == 0 && p.N % BN == 0 &&
+                       epilogue_frag_ok(e, 0, 0, plan.bm, BN, H);
+  if (persist) return plan.bm == 256 ? launch_tc_major<256, 128, true, true>(amn, bmn, ah, al, bh, bl, e, splits, st)
+                                     : launch_tc_major<128, 128, true, true>(amn, bmn, ah, al, bh, bl, e, splits, st);
   if (H) {
     if (plan.bm == 256) return BN == 128 ? launch_tc_major<256, 128, true>(amn, bmn, ah, al, bh, bl, e, splits, st)
                                          : launch_tc_major<256, 64, true>(amn, bmn, ah, al, bh, bl, e, splits, st);

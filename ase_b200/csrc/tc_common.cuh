@@ -216,7 +216,8 @@ struct TcEpi {
   int skip_c;                              // the planes are the only consumers of C: no fp32 store
   int debug;   // experiments only (env ASE_TC_DEBUG): 1 skip the whole store phase, 4 skip correction MMAs,
                // 16 skip mask loads, 32 skip plane stores, 64 skip column-sum atomics, 128 skip the fp32 C store,
-               // 256 generic store phase only, 512 pin the tile height to 128 rows (gemm_tc_plan)
+               // 256 generic store phase only, 512 pin the tile height to 128 rows (gemm_tc_plan),
+               // 1024 one tile per CTA (no persistent tile loop)
 };
 
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {

@@ -7,7 +7,10 @@
                                                        subprocess: the library reads the bits once per process)
   python tools/bench_gemm.py [backend] --minibatch --store-share
                                                        the second column is the same shape with the store phase dropped
-                                                       (ASE_TC_DEBUG bit 1) instead: what the store phase costs per shape"""
+                                                       (ASE_TC_DEBUG bit 1) instead: what the store phase costs per shape
+  python tools/bench_gemm.py [backend] --minibatch --persistent
+                                                       the second column is the same shape on the one-tile-per-CTA kernel
+                                                       (ASE_TC_DEBUG bit 1024) instead of the persistent one"""
 import ctypes as C
 import json
 import os
@@ -123,7 +126,8 @@ if '--minibatch' in sys.argv:
     if '--json' in sys.argv:
         print(json.dumps(rows))
         sys.exit(0)
-    other_bit, other = (1, 'no store') if '--store-share' in sys.argv else (512, 'pinned 128')
+    other_bit, other = ((1, 'no store') if '--store-share' in sys.argv else (1024, 'tile/CTA') if '--persistent' in sys.argv
+                        else (512, 'pinned 128'))
     env = dict(os.environ, ASE_TC_DEBUG=str(int(os.environ.get('ASE_TC_DEBUG', '0')) | other_bit))
     r = subprocess.run([sys.executable, os.path.abspath(__file__), str(backend), '--minibatch', '--json'], env=env, capture_output=True, text=True)
     pinned = json.loads(r.stdout.strip().splitlines()[-1]) if r.returncode == 0 else None
